@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""Benchmark of the MagicPose DDIM denoising hot path on B200 (contract: see the task statement).
+"""Benchmark of the MagicPose DDIM denoising hot path on one or more H100s.
 
     python bench.py --gpus 1 --steps 50 --warmup 3            # ours, one frame, full 50-step chain
     torchrun --nproc-per-node N ... bench.py --gpus N ...     # frames sharded over N GPUs
     python bench.py --impl reference --steps K --warmup W     # the reference's path on the host CPUs
+    python bench.py --gpus 1 --steps 5 --warmup 1 --dump-outputs DIR   # also write the last step's outputs as .npy
 
 A "step" is one p_sample_ddim (ddim.py:518-645) for the per-GPU batch of frames: the pose
 ControlNet, the UNet in 'read' mode with the appearance bank, the unconditional UNet, CFG combine
@@ -24,6 +25,10 @@ What one run reports (rank 0 prints ONE JSON line):
                         and within fp16 tolerance of rank 0's chain with a locally built bank
   gpu_eager_baseline    (N = 1) the reference's modules as eager PyTorch (cuDNN/cuBLAS/SDPA, fp16 autocast) on this GPU
   cpu_baseline          (N = 1) the oracle port of the same step on the host cores
+
+--dump-outputs DIR writes, after the timed steps of the headline measurement, what its last step returned to the caller:
+x_prev.npy and pred_x0.npy (fp32 [B, 4, latent, latent], rank 0).  Inputs and weights are seeded, so two builds run with
+the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -63,13 +68,15 @@ def parse():
     ap.add_argument("--no-config4", action="store_true", help="skip the configs[3] sub-record and the probe (N > 1)")
     ap.add_argument("--nvtx", action="store_true", help="wrap the LAST step of the steady-state run in an NVTX range "
                     "'mdb_step' (ncu --nvtx --nvtx-include 'mdb_step/' then profiles exactly one step)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline run's last-step outputs (x_prev, pred_x0) as DIR/<name>.npy, float32")
     ap.add_argument("--tune", default="", help="experiments: launch heuristics as k=v[,k=v] (keys of ops.tuning)")
     return ap.parse_args()
 
 
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -218,7 +225,7 @@ def roofline_probe(torch, ops, trace, peaks, frames_per_gpu=1):
         tot_t += t * c
         rows.append((fl * c, t * c, (m, n, k, conv is not None, splits), c))
     rows.sort(key=lambda r: -r[1])
-    peak = peaks.get("bf16_tflops", 1590.0)
+    peak = peaks.get("bf16_tflops", 989.0)  # H100 SXM data sheet, dense FP16/BF16
     ach = tot_fl / tot_t / 1e12
     top = [{"shape_mnk_conv_splits": list(map(int, r[2][:3])) + [bool(r[2][3]), int(r[2][4])], "count": r[3],
             "ms_total": r[1] * 1e3, "tflops": r[0] / r[1] / 1e12} for r in rows[:6]]
@@ -233,9 +240,9 @@ def roofline_probe(torch, ops, trace, peaks, frames_per_gpu=1):
             traffic = float(traffic_detail["dram_bytes_per_launch_avg"])
     except Exception:  # noqa: BLE001
         traffic, traffic_detail = None, None
-    return {"bound": "tensor", "kernel": "gemm_tc_kernel (tcgen05 GEMM + 3x3 implicit-GEMM conv)",
+    return {"bound": "tensor", "kernel": "gemm_tc_kernel (wgmma GEMM + 3x3 implicit-GEMM conv)",
             "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
-            "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst)" if "bf16_tflops" in peaks else "fallback 1590",
+            "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst)" if "bf16_tflops" in peaks else "H100 SXM data sheet 989 (dense)",
             "traffic": traffic, "traffic_detail": traffic_detail, "gemm_gflop_per_step": tot_fl / 1e9,
             "gemm_ms_per_step_isolated": tot_t * 1e3, "launches_per_step": int(sum(cnt.values())), "top_by_time": top}
 
@@ -350,6 +357,7 @@ class Bench:
         x_final = run(K)
         e1.record()
         self.barrier()
+        outputs = {"x_prev": gd.x_prev.float().cpu().numpy(), "pred_x0": gd.pred_x0.float().cpu().numpy()}
         launches = ops.launch_count() + gd.replayed_launches - l0
         sec = self.max_over_ranks(e0.elapsed_time(e1)) * 1e-3
         clk = clocks.stop()
@@ -359,9 +367,9 @@ class Bench:
         rec = {"frames_per_gpu": B, "value": world * B * K / sec, "unit": UNIT, "ms_per_step": sec * 1e3 / K, "steps": K,
                "bank_build_ms": bank_ms, "bank_chunk": chunk, "gpu_launches": int(launches), "clocks": clk,
                "finite": finite, "x_final_fingerprint": fp, "step_launches": int(gd.step_launches),
-               "bank_launches": int(gd.bank_launches)}
+               "bank_launches": int(gd.bank_launches), "outputs": outputs}
         gflop = GF_FRAME_STEP * B * K * world + GF_REF_STEP * uniq_n
-        peak_s = self.peaks.get("bf16_tflops_sustained", 1400.0)
+        peak_s = self.peaks.get("bf16_tflops_sustained", 989.0)
         rec["step_roofline"] = {"algorithmic_gflop": gflop, "achieved_tflops": gflop / sec / 1e3,
                                 "peak_tflops_per_gpu": peak_s, "frac": gflop / sec / 1e3 / (world * peak_s)}
         if world > 1:
@@ -506,6 +514,12 @@ def run_ours(args):
     K, W, B = args.steps, args.warmup, args.batch
     # N > 1: the ranks hold frames of ONE sequence (shared reference image / prompt / x_T, own pose maps)
     main = b.measure(B, K, W, e2e=not args.no_e2e, sequence_frames=world > 1)
+    outputs = main.pop("outputs")
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in outputs.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
     roof = None
     if rank == 0 and not args.no_roofline:
         roof = b.roofline(B)
@@ -517,11 +531,13 @@ def run_ours(args):
             torch.cuda.empty_cache()
             # BASELINE configs[3]: one sequence, 8 frames per GPU (64 over 8 GPUs), bank sharded + gathered in the timer
             cfg4 = b.measure(8, K, W, e2e=not args.no_e2e, sequence_frames=True)
+            cfg4.pop("outputs")
     batch8 = None
     if world == 1 and B != 8 and not args.no_batch8:
         b._last = None
         torch.cuda.empty_cache()
         batch8 = b.measure(8, K, W, e2e=not args.no_e2e)
+        batch8.pop("outputs")
         if not args.no_roofline:
             batch8["roofline"] = b.roofline(8)
 
@@ -540,7 +556,7 @@ def run_ours(args):
                    "bank": "appearance pass once per timestep per sequence (timesteps batched %d at a time, sharded "
                            "over ranks + one all-gather per slot row, overlapped with the first steps), inside the "
                            "timed region" % main["bank_chunk"],
-                   "l2": "no flush needed: each step streams >4 GB of fp16 weights (L2 is 126 MB)",
+                   "l2": "no flush needed: each step streams >4 GB of fp16 weights (L2 is 50 MB)",
                    "weights": "random init (seeded), fp16 storage, fp32 accumulate",
                    "cuda_graph": True, **({"tune": args.tune} if args.tune else {})},
         "gpu_launches": main["gpu_launches"], "clocks": main["clocks"], "finite": main["finite"],
@@ -553,7 +569,7 @@ def run_ours(args):
     if roof is not None:
         line["roofline"] = roof
     if batch8 is not None:
-        batch8["config"] = "512x512, 50-step DDIM, batch 8, fp16, 1xB200 (BASELINE.json configs[2])"
+        batch8["config"] = "512x512, 50-step DDIM, batch 8, fp16, 1xH100 (BASELINE.json configs[2])"
         line["batch8"] = batch8
     if cfg4 is not None:
         cfg4["config"] = ("%d-frame pose sequence, shared reference image, 8 frames per GPU over %d GPUs, bank sharded "

@@ -1,5 +1,5 @@
 /*
- * magicdance_b200 — C ABI of the B200 (sm_100a) kernels behind MagicPose's DDIM denoising hot path.
+ * magicdance_b200 — C ABI of the H100 (sm_90a) kernels behind MagicPose's DDIM denoising hot path.
  *
  * The reference (Boese0601/MagicDance) has no FFI: its "plugin API" is Python classes looked up by
  * YAML `target:` strings (model_lib/ControlNet/ldm/util.py:72-87).  The drop-in Python classes in
@@ -14,7 +14,7 @@
  *   - weights are fp16, "K-major": Linear (out,in) as is; Conv2d OIHW repacked to [O][kh][kw][I];
  *   - `stream` is a cudaStream_t (0 = legacy default stream); every call is asynchronous;
  *   - return value: 0 on success, negative MDB_ERR_* otherwise; mdb_last_error() gives the text.
- *   - there is NO CPU fallback: without an sm_100 device every compute entry returns an error.
+ *   - there is NO CPU fallback: without an sm_90 device every compute entry returns an error.
  */
 #ifndef MAGICDANCE_B200_H_
 #define MAGICDANCE_B200_H_
@@ -44,16 +44,16 @@ int64_t mdb_launch_count(void);
 /* sizeof(mdb_gemm_desc) (which = 0) / sizeof(mdb_attn_desc) (which = 1): a binding checks its struct mirrors */
 int64_t mdb_abi_struct_bytes(int32_t which);
 
-/* Launch heuristics, process-wide.  The defaults are what the B200 measurements selected (profiles/); tests use the
- * setter to force a kernel variant onto small problems. */
-#define MDB_TUNE_GEMM_PAIR_MIN_TILES 1 /* grids of >= this many 128-row tiles use the persistent CTA-pair GEMM (128) */
-#define MDB_TUNE_ATTN40_2Q_MIN_CTAS 3  /* d=40 attention grids of >= this many CTAs use the two-Q-tile kernel (2048) */
+/* Launch heuristics, process-wide (defaults in parentheses); tests use the setter to force a kernel variant onto small
+ * problems. */
+#define MDB_TUNE_GEMM_PAIR_MIN_TILES 1 /* grids of >= this many tiles use the one-CTA-per-SM large-grid tiles (128) */
+#define MDB_TUNE_ATTN40_2Q_MIN_CTAS 3  /* d=40 attention grids of >= this many CTAs run two CTAs per SM (512) */
 #define MDB_TUNE_GEMM_BN80_BELOW 4     /* N %% 160 == 0 layers with fewer 160-wide CTAs than this take 80-wide tiles (100) */
 int mdb_set_tuning(int32_t key, int32_t value);
 int32_t mdb_get_tuning(int32_t key);
 
 /* ------------------------------------------------------------------------------------------------
- * Tensor-core GEMM / implicit-GEMM convolution (tcgen05 + TMEM + TMA).
+ * Tensor-core GEMM / implicit-GEMM convolution (wgmma + TMA).
  *   D[M,N] = epilogue( A[M,K] * B[N,K]^T )     fp16 in, fp32 accumulate, fp16 out
  * Replaces: nn.Linear in CrossAttention.to_q/to_k/to_v/to_out (ldm/modules/attention.py:154-161),
  * GEGLU.proj / FeedForward.net[2] (attention.py:53-56,68-72), the 1x1 convs proj_in/proj_out
@@ -98,7 +98,7 @@ typedef struct mdb_gemm_desc {
 int mdb_gemm_f16(const mdb_gemm_desc* desc, mdb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Fused attention, FlashAttention-style tile loop on tcgen05, with TWO key/value sources whose
+ * Fused attention, FlashAttention-style tile loop on wgmma, with TWO key/value sources whose
  * keys are concatenated in-kernel:  out = softmax([Q K0^T | Q K1^T] * scale) [V0 ; V1].
  * Replaces CrossAttention._forward (attention.py:168-199) / MemoryEfficientCrossAttention
  * (attention.py:225-250) AND the torch.cat([x_norm1] + bank) of BasicTransformerBlock 'read'

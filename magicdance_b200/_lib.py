@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI declared in include/magicdance_b200.h.
 
 There is deliberately no fallback: if the shared library is missing or the device is not
-sm_100, every compute entry point raises.
+sm_90, every compute entry point raises.
 """
 from __future__ import annotations
 

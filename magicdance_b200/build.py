@@ -1,4 +1,4 @@
-"""Builds the sm_100a kernel library (C ABI, include/magicdance_b200.h) in-tree with nvcc.
+"""Builds the sm_90a kernel library (C ABI, include/magicdance_b200.h) in-tree with nvcc.
 
 nvcc cross-compiles without a GPU, so this runs in the CPU-only build container; the resulting
 magicdance_b200/lib/libmagicdance_b200.so travels to the GPU box with the repo snapshot.
@@ -16,9 +16,9 @@ LIB_DIR = os.path.join(PKG, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libmagicdance_b200.so")
 STAMP = os.path.join(LIB_DIR, "build.stamp")
 SOURCES = ["gemm.cu", "attention.cu", "norm.cu", "misc.cu"]
-HEADERS = ["common.cuh", os.path.join("..", "..", "include", "magicdance_b200.h")]
+HEADERS = ["common.cuh", "wgmma.cuh", os.path.join("..", "..", "include", "magicdance_b200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 

@@ -1,5 +1,5 @@
-// Fused attention for sm_100a: softmax([Q K0^T | Q K1^T] * scale) [V0 ; V1], FlashAttention-style
-// online softmax, both GEMMs on tcgen05 with TMEM accumulators, operands fed by TMA.
+// Fused attention for sm_90a: softmax([Q K0^T | Q K1^T] * scale) [V0 ; V1], FlashAttention-style
+// online softmax, both GEMMs on wgmma with register accumulators, operands fed by TMA.
 //
 // The two key/value sources are the layer's own tokens (source 0) and the appearance bank
 // (source 1): the reference concatenates them with torch.cat before to_k/to_v
@@ -7,14 +7,15 @@
 // source 1's, so no concatenated K/V buffer ever exists.
 //
 // One CTA = 128 queries x 1 head x 1 batch element.  Warp roles:
-//   warp 0     TMA producer: Q once; K tile [BKV][d] and V^T tile [d][BKV] per step, 2-stage ring.
+//   warp 8     TMA producer: Q once; K tile [BKV][d] and V^T tile [d][BKV] per step, STAGES-deep ring.
 //              Head slices are cut out of the [tokens][heads*d] activations by a 3-D tensor map
 //              (d, heads, tokens) whose innermost extent is d, so the 64-wide box is zero-filled
-//              beyond d — that is the K-dim padding 40->48 / 80->128 / 160->192 for free.
-//   warp 1     MMA issuer: S = Q K^T (M=128, N=BKV) into TMEM; after the softmax warps publish P
-//              (fp16, smem, 128B-swizzled K-major) O += P V (M=128, N=DV) into TMEM.
-//   warps 2-5  softmax: thread == query row.  tcgen05.ld S, running max / sum in the log2 domain,
-//              lazy O rescale (only when the max grows by > 2^8), write P, final O / l -> fp16.
+//              beyond d — that is the K-dim padding 40->48 / 80->80 / 160->192 for free.
+//   warps 0-7  two warpgroups of 64 query rows each.  Per key tile: S = Q K^T (wgmma, M=64, N=BKV, both
+//              operands in shared memory) into registers; running max / sum in the log2 domain over the
+//              four threads that share a row; P = exp2(S - max) is rounded to fp16 IN REGISTERS, in exactly
+//              the fragment layout the register-A form of wgmma takes, and O += P V^T (N = d rounded up to
+//              16) accumulates in registers.  O / l -> fp16 at the end.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -22,52 +23,27 @@
 namespace mdb {
 
 int get_attn_tuning();
+void count_launch(int n = 1);
 void set_attn_tuning(int v);
 
-constexpr int kAttnThreads = 192;
+constexpr int kAttnConsumers = 256;                 // warpgroups 0 and 1
+constexpr int kAttnProducerWarp = kAttnConsumers / 32;
+constexpr int kAttnThreads = kAttnConsumers + 32;
 constexpr int kBQ = 128;
 
-template <int D, int BKV>
+template <int D, int BKV, int STAGES>
 struct AttnCfg {
   static constexpr int kDkChunks = (D + 63) / 64;
   static constexpr int kDV = (D + 15) / 16 * 16;  // PV N and number of QK K-steps * 16
   static constexpr int kKSteps = kDV / 16;
-  static constexpr int kKvChunks = BKV / 64;
   static constexpr int kQBytes = kDkChunks * kBQ * 128;
   static constexpr int kKBytes = kDkChunks * BKV * 128;
-  static constexpr int kVBytes = kKvChunks * kDV * 128;
-  // Row sums on the tensor core: when the PV tile has at least 8 spare rows (d = 40 -> 48), the 8-row swizzle group
-  // [D, D+8) of every V^T stage tile is never written by TMA (the box is D rows) and is pre-filled once per CTA with
-  // row D = ones, rows D+1.. = zeros — so O[:, D] accumulates sum_k P[:, k], the softmax denominator, in the same
-  // MMAs that produce O, and the softmax warps do not sum P at all (64 FADD of ~500 instructions per 128x64 tile).
-  static constexpr bool kOnes = (kDV - D >= 8) && (D % 8 == 0);
-  static constexpr int kVRowsTma = kOnes ? D : kDV;
-  static constexpr int kVBytesTma = kKvChunks * kVRowsTma * 128;
-  static constexpr int kPBytes = kKvChunks * kBQ * 128;
-  static constexpr int kStages = 2;
-  static constexpr int kSmem = kQBytes + kStages * (kKBytes + kVBytes) + kPBytes + 1024;
-  static constexpr int kTmemCols = (BKV + kDV <= 128) ? 128 : (BKV + kDV <= 256 ? 256 : 512);
-  static constexpr int kOCol = BKV;  // O accumulator starts after S
+  static constexpr int kVBytes = kDV * 128;         // one 64-key chunk of V^T: [kDV rows][64 keys]
+  static constexpr int kStageBytes = kKBytes + kVBytes;
+  static constexpr int kSmem = kQBytes + STAGES * kStageBytes + 1024;
+  static_assert(BKV == 64, "one 128-byte swizzle row of keys per V^T tile");
+  static_assert(kVBytes % 1024 == 0 && kKBytes % 1024 == 0, "stage tiles start on swizzle-atom boundaries");
 };
-
-// rows [D, D+8) of every V^T stage tile <- (ones, zeros x 7); called by the non-producer warps before the CTA barrier
-template <typename C1, int D, int STAGES>
-__device__ __forceinline__ void attn_fill_ones_rows(uint8_t* sKV, int stage_bytes, int k_bytes, int tid, int nthreads) {
-  if constexpr (C1::kOnes) {
-    for (int i = tid; i < STAGES * C1::kKvChunks * 64; i += nthreads) {  // 64 16-byte pieces per 1 KB swizzle group
-      const int piece = i & 63, grp = i >> 6;
-      const int stage = grp / C1::kKvChunks, kc = grp % C1::kKvChunks;
-      uint8_t* g = sKV + stage * stage_bytes + k_bytes + kc * (C1::kDV * 128) + (D / 8) * 1024;
-      const uint32_t v = (piece < 8) ? 0x3C003C00u : 0u;  // row 0 of the group (pieces 0..7) = fp16 1.0 x 64
-      *reinterpret_cast<uint4*>(g + piece * 16) = make_uint4(v, v, v, v);
-    }
-    fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's reads of shared memory
-  }
-}
-
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint4 v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
 
 struct AttnKParams {
   CUtensorMap tmQ, tmK0, tmV0, tmK1, tmV1;
@@ -80,645 +56,46 @@ struct AttnKParams {
   float scale_log2;
 };
 
-template <int D, int BKV>
-__global__ void __launch_bounds__(kAttnThreads, (D <= 80) ? 2 : 1) attn_tc_kernel(const __grid_constant__ AttnKParams p) {
-  using C = AttnCfg<D, BKV>;
+// MINB = 2 caps the registers so that two CTAs (four MMA warpgroups) share an SM.
+template <int D, int BKV, int STAGES, int MINB>
+__global__ void __launch_bounds__(kAttnThreads, MINB) attn_wg_kernel(const __grid_constant__ AttnKParams p) {
+  using C = AttnCfg<D, BKV, STAGES>;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t q_bar, s_full, p_full, o_done;
-  __shared__ __align__(8) uint64_t kv_full[C::kStages], kv_empty[C::kStages];
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ __align__(8) uint64_t q_bar;
+  __shared__ __align__(8) uint64_t kv_full[STAGES], kv_empty[STAGES];
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
   uint8_t* sKV = sQ + C::kQBytes;
-  uint8_t* sP = sKV + C::kStages * (C::kKBytes + C::kVBytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * kBQ;
   const int head = blockIdx.y;
   const int b = blockIdx.z;
-
   const int t0 = (p.n0 + BKV - 1) / BKV;
   const int t1 = (b < p.bank_batches && p.n1 > 0) ? (p.n1 + BKV - 1) / BKV : 0;
   const int n_tiles = t0 + t1;
 
   pdl_launch_dependents();
-  if (warp == 0 && lane == 0) {
+  if (warp == kAttnProducerWarp && lane == 0) {
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK0);
     tma_prefetch_desc(&p.tmV0);
     mbar_init(&q_bar, 1);
-    mbar_init(&s_full, 1);
-    mbar_init(&p_full, 128);
-    mbar_init(&o_done, 1);
-    for (int s = 0; s < C::kStages; ++s) {
+    for (int s = 0; s < STAGES; ++s) {
       mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
+      mbar_init(&kv_empty[s], kAttnConsumers);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, C::kTmemCols);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_smem;
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == kAttnProducerWarp) {
     if (lane == 0) {
       mbar_expect_tx(&q_bar, C::kQBytes);
       for (int dc = 0; dc < C::kDkChunks; ++dc)
-        tma_load_3d(sQ + dc * (kBQ * 128), &p.tmQ, &q_bar, dc * 64, head, b * p.nq + q0);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j % C::kStages;
-        const uint32_t ph = (j / C::kStages) & 1;
-        const bool src1 = j >= t0;
-        const int key0 = (src1 ? (j - t0) : j) * BKV;
-        const CUtensorMap* tk = src1 ? &p.tmK1 : &p.tmK0;
-        const CUtensorMap* tv = src1 ? &p.tmV1 : &p.tmV0;
-        const int nsrc = src1 ? p.n1 : p.n0;
-        const int kvb = src1 ? (p.kv1_batches > 1 ? b : 0) : (p.kv0_batches > 1 ? b : 0);
-        const int ldvb = src1 ? p.ldv1_batch : p.ldv0_batch;
-        mbar_wait(&kv_empty[s], ph ^ 1);
-        mbar_expect_tx(&kv_full[s], C::kKBytes + C::kVBytes);
-        uint8_t* sk = sKV + s * (C::kKBytes + C::kVBytes);
-        uint8_t* sv = sk + C::kKBytes;
-        for (int dc = 0; dc < C::kDkChunks; ++dc)
-          tma_load_3d(sk + dc * (BKV * 128), tk, &kv_full[s], dc * 64, head, kvb * nsrc + key0);
-        for (int kc = 0; kc < C::kKvChunks; ++kc)
-          tma_load_2d(sv + kc * (C::kDV * 128), tv, &kv_full[s], kvb * ldvb + key0 + kc * 64, head * D);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = umma_idesc_f16(kBQ, BKV);
-      constexpr uint32_t idesc_pv = umma_idesc_f16(kBQ, C::kDV);
-      const uint32_t q_addr = smem_u32(sQ);
-      const uint32_t p_addr = smem_u32(sP);
-      mbar_wait(&q_bar, 0);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j % C::kStages;
-        const uint32_t ph = (j / C::kStages) & 1;
-        mbar_wait(&kv_full[s], ph);
-        tc_fence_after_sync();
-        const uint32_t k_addr = smem_u32(sKV + s * (C::kKBytes + C::kVBytes));
-        const uint32_t v_addr = k_addr + C::kKBytes;
-        // S = Q K^T : K-steps of 16 over the (zero-padded) head dim
-#pragma unroll
-        for (int ks = 0; ks < C::kKSteps; ++ks) {
-          const int dc = ks >> 2, kk = ks & 3;
-          const uint64_t da = umma_desc_k_sw128(q_addr + dc * (kBQ * 128)) + 2 * kk;
-          const uint64_t db = umma_desc_k_sw128(k_addr + dc * (BKV * 128)) + 2 * kk;
-          umma_f16_ss(tmem_base, da, db, idesc_qk, ks != 0 ? 1u : 0u);
-        }
-        umma_commit(&s_full);
-        // wait for P(j) (and the O rescale) from the softmax warps
-        mbar_wait(&p_full, j & 1);
-        tc_fence_after_sync();
-#pragma unroll
-        for (int ks = 0; ks < BKV / 16; ++ks) {
-          const int kc = ks >> 2, kk = ks & 3;
-          const uint64_t da = umma_desc_k_sw128(p_addr + kc * (kBQ * 128)) + 2 * kk;
-          const uint64_t db = umma_desc_k_sw128(v_addr + kc * (C::kDV * 128)) + 2 * kk;
-          umma_f16_ss(tmem_base + C::kOCol, da, db, idesc_pv, (j | ks) != 0 ? 1u : 0u);
-        }
-        umma_commit(&kv_empty[s]);
-        umma_commit(&o_done);
-      }
-    }
-  } else {
-    // ---------------- softmax / correction / epilogue warps ----------------
-    const int g = warp & 3;
-    const int r = g * 32 + lane;  // query row inside the tile == TMEM lane
-    const uint32_t t_s = tmem_base + (static_cast<uint32_t>(g * 32) << 16);
-    const uint32_t t_o = t_s + C::kOCol;
-    float m_run = -INFINITY;
-    float l_run = 0.f;
-    uint8_t* p_row = sP + (r >> 3) * 1024 + (r & 7) * 128;
-    const int sw = r & 7;
-
-    for (int j = 0; j < n_tiles; ++j) {
-      const bool src1 = j >= t0;
-      const int key0 = (src1 ? (j - t0) : j) * BKV;
-      const int valid = min(BKV, (src1 ? p.n1 : p.n0) - key0);
-      mbar_wait(&s_full, j & 1);
-      tc_fence_after_sync();
-      // pass 1 over S (TMEM reads are cheap): raw row max; the softmax scale is positive, so it is applied
-      // to the max afterwards.  The unmasked path costs half an instruction per element (3-input max).
-      float mt = -INFINITY;
-      if (valid == BKV) {
-#pragma unroll
-        for (int c = 0; c < BKV / 32; ++c) {
-          uint32_t rr[32];
-          tmem_ld_x32(t_s + c * 32, rr);
-          tmem_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) mt = fmax3(mt, __uint_as_float(rr[i]), __uint_as_float(rr[i + 1]));
-        }
-      } else {
-#pragma unroll
-        for (int c = 0; c < BKV / 32; ++c) {
-          uint32_t rr[32];
-          tmem_ld_x32(t_s + c * 32, rr);
-          tmem_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (c * 32 + i < valid) mt = fmaxf(mt, __uint_as_float(rr[i]));
-        }
-      }
-      mt *= p.scale_log2;
-      float m_new = m_run;
-      if (mt - m_run > 8.0f) m_new = mt;  // lazy: tolerate p <= 2^8 before paying for a rescale
-      const float alpha = ex2_approx(m_run - m_new);  // m_run = -inf on the first tile -> 0
-      m_run = m_new;
-
-      if (j > 0) {
-        // PV(j-1) must have finished before P is overwritten / O is rescaled
-        mbar_wait(&o_done, (j - 1) & 1);
-        tc_fence_after_sync();
-        if (__any_sync(0xffffffffu, alpha != 1.0f)) {
-#pragma unroll
-          for (int c = 0; c < C::kDV / 16; ++c) {
-            uint32_t oo[16];
-            tmem_ld_x16(t_o + c * 16, oo);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) oo[i] = __float_as_uint(__uint_as_float(oo[i]) * alpha);
-            tmem_st_x16(t_o + c * 16, oo);
-          }
-          tmem_wait_st();
-        }
-      }
-      // pass 2: p = exp2(s - m), row sum, P -> smem (K-major 128B-swizzled: 16-byte unit u of row r
-      // lands at unit u ^ (r & 7)).  32 columns at a time keeps the live register set small enough for
-      // two CTAs per SM, which is what overlaps one CTA's softmax with the other's MMAs.
-      float ls0 = 0.f, ls1 = 0.f, ls2 = 0.f, ls3 = 0.f;
-      const float neg_m = -m_new;
-#pragma unroll
-      for (int c = 0; c < BKV / 32; ++c) {
-        uint32_t rr[32];
-        tmem_ld_x32(t_s + c * 32, rr);
-        tmem_wait_ld();
-        float pv[32];
-        if (valid == BKV) {  // one FFMA + one MUFU.EX2 + one FADD per element
-#pragma unroll
-          for (int i = 0; i < 32; ++i) pv[i] = ex2_approx(fmaf(__uint_as_float(rr[i]), p.scale_log2, neg_m));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            pv[i] = (c * 32 + i < valid) ? ex2_approx(fmaf(__uint_as_float(rr[i]), p.scale_log2, neg_m)) : 0.f;
-        }
-#pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          ls0 += pv[i]; ls1 += pv[i + 1]; ls2 += pv[i + 2]; ls3 += pv[i + 3];
-        }
-#pragma unroll
-        for (int u4 = 0; u4 < 4; ++u4) {
-          uint4 pk;
-          pk.x = pack_half2(pv[u4 * 8 + 0], pv[u4 * 8 + 1]);
-          pk.y = pack_half2(pv[u4 * 8 + 2], pv[u4 * 8 + 3]);
-          pk.z = pack_half2(pv[u4 * 8 + 4], pv[u4 * 8 + 5]);
-          pk.w = pack_half2(pv[u4 * 8 + 6], pv[u4 * 8 + 7]);
-          const int u = c * 4 + u4;
-          const int kc = u >> 3, uu = u & 7;
-          *reinterpret_cast<uint4*>(p_row + kc * (kBQ * 128) + ((uu ^ sw) << 4)) = pk;
-        }
-      }
-      const float lsum = (ls0 + ls1) + (ls2 + ls3);
-      l_run = l_run * alpha + lsum;
-      fence_proxy_async_smem();
-      tc_fence_before_sync();
-      mbar_arrive(&p_full);
-    }
-
-    // final: O / l -> fp16
-    mbar_wait(&o_done, (n_tiles - 1) & 1);
-    tc_fence_after_sync();
-    const float inv_l = 1.0f / l_run;
-    const int q = q0 + r;
-    __half* op = p.out + (static_cast<long long>(b) * p.nq + q) * p.ldo + head * D;
-#pragma unroll
-    for (int c = 0; c < C::kDV / 16; ++c) {
-      uint32_t oo[16];
-      tmem_ld_x16(t_o + c * 16, oo);
-      tmem_wait_ld();
-      if (q < p.nq) {
-#pragma unroll
-        for (int h8 = 0; h8 < 2; ++h8) {
-          if (c * 16 + h8 * 8 < D) {
-            uint4 o4;
-            o4.x = pack_half2(__uint_as_float(oo[h8 * 8 + 0]) * inv_l, __uint_as_float(oo[h8 * 8 + 1]) * inv_l);
-            o4.y = pack_half2(__uint_as_float(oo[h8 * 8 + 2]) * inv_l, __uint_as_float(oo[h8 * 8 + 3]) * inv_l);
-            o4.z = pack_half2(__uint_as_float(oo[h8 * 8 + 4]) * inv_l, __uint_as_float(oo[h8 * 8 + 5]) * inv_l);
-            o4.w = pack_half2(__uint_as_float(oo[h8 * 8 + 6]) * inv_l, __uint_as_float(oo[h8 * 8 + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(op + c * 16 + h8 * 8) = o4;
-          }
-        }
-      }
-    }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, C::kTmemCols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// v2: two Q tiles (256 queries) per CTA, ping-pong.  One K/V tile feeds both Q tiles; each Q tile has
-// its own S and O accumulators in TMEM, its own P buffer and its own softmax warpgroup (warps 2-5 for
-// tile A, 6-9 for tile B).  The MMA thread interleaves the two tiles — PV_A(j), QK_A(j+1), PV_B(j),
-// QK_B(j+1) — so while warpgroup A runs its softmax the tensor core works for B and vice versa, and
-// the MUFU (exp2) pipe, which bounds d=40 attention, always has a warpgroup feeding it.
-// TMEM columns: S_A [0,BKV) S_B [BKV,2BKV) O_A [2BKV,2BKV+DV) O_B [2BKV+DV, 2BKV+2DV)  (<= 512).
-// ------------------------------------------------------------------------------------------------
-constexpr int kAttn2Threads = 320;
-
-template <int D, int BKV>
-struct Attn2Cfg {
-  using C1 = AttnCfg<D, BKV>;
-  static constexpr int kDV = C1::kDV;
-  static constexpr int kQBytes = C1::kQBytes;   // per Q tile
-  static constexpr int kKBytes = C1::kKBytes;
-  static constexpr int kVBytes = C1::kVBytes;
-  static constexpr int kPBytes = C1::kPBytes;   // per Q tile
-  static constexpr int kStages = 2;
-  static constexpr int kSmem = 2 * kQBytes + kStages * (kKBytes + kVBytes) + 2 * kPBytes + 1024;
-  static constexpr int kCols = 2 * BKV + 2 * kDV;
-  static constexpr int kTmemCols = kCols <= 256 ? 256 : 512;
-  static_assert(kCols <= 512, "TMEM budget");
-};
-
-// MINB = 2 (d=40 with 64-key tiles: 224 TMEM columns, 93 KB of shared memory) puts TWO such CTAs on an SM —
-// 16 softmax warps instead of the 8 of the one-Q-tile kernel at two CTAs per SM; the register cap becomes
-// 65536 / 640 = 102 per thread.  Used for large grids (mdb_attention_f16: >= 2048 CTAs at d=40; MINB = 1 at d=80
-// from 512 CTAs, where the one-Q-tile kernel only fits one CTA = four softmax warps per SM).
-template <int D, int BKV, int MINB = 1>
-__global__ void __launch_bounds__(kAttn2Threads, MINB) attn2_tc_kernel(const __grid_constant__ AttnKParams p) {
-  using C = Attn2Cfg<D, BKV>;
-  using C1 = AttnCfg<D, BKV>;
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t q_bar;
-  __shared__ __align__(8) uint64_t s_full[2], p_full[2], o_done[2];
-  __shared__ __align__(8) uint64_t kv_full[C::kStages], kv_empty[C::kStages];
-  __shared__ uint32_t tmem_base_smem;
-
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                                   // [2][kQBytes]
-  uint8_t* sKV = sQ + 2 * C::kQBytes;                   // [stages][K | V]
-  uint8_t* sP = sKV + C::kStages * (C::kKBytes + C::kVBytes);  // [2][kPBytes]
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * (2 * kBQ);
-  const int head = blockIdx.y;
-  const int b = blockIdx.z;
-  const bool tile_b_active = q0 + kBQ < p.nq;  // CTA-uniform
-
-  const int t0 = (p.n0 + BKV - 1) / BKV;
-  const int t1 = (b < p.bank_batches && p.n1 > 0) ? (p.n1 + BKV - 1) / BKV : 0;
-  const int n_tiles = t0 + t1;
-
-  pdl_launch_dependents();
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.tmQ);
-    tma_prefetch_desc(&p.tmK0);
-    tma_prefetch_desc(&p.tmV0);
-    mbar_init(&q_bar, 1);
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&s_full[t], 1);
-      mbar_init(&p_full[t], 128);
-      mbar_init(&o_done[t], 1);
-    }
-    for (int s = 0; s < C::kStages; ++s) {
-      mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, C::kTmemCols);
-  if (warp >= 2)
-    attn_fill_ones_rows<C1, D, C::kStages>(sKV, C::kKBytes + C::kVBytes, C::kKBytes, threadIdx.x - 64, kAttn2Threads - 64);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_smem;
-  pdl_wait();
-
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(&q_bar, 2 * C::kQBytes);
-      for (int t = 0; t < 2; ++t)
-        for (int dc = 0; dc < C1::kDkChunks; ++dc)
-          tma_load_3d(sQ + t * C::kQBytes + dc * (kBQ * 128), &p.tmQ, &q_bar, dc * 64, head, b * p.nq + q0 + t * kBQ);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j % C::kStages;
-        const uint32_t ph = (j / C::kStages) & 1;
-        const bool src1 = j >= t0;
-        const int key0 = (src1 ? (j - t0) : j) * BKV;
-        const CUtensorMap* tk = src1 ? &p.tmK1 : &p.tmK0;
-        const CUtensorMap* tv = src1 ? &p.tmV1 : &p.tmV0;
-        const int nsrc = src1 ? p.n1 : p.n0;
-        const int kvb = src1 ? (p.kv1_batches > 1 ? b : 0) : (p.kv0_batches > 1 ? b : 0);
-        const int ldvb = src1 ? p.ldv1_batch : p.ldv0_batch;
-        mbar_wait(&kv_empty[s], ph ^ 1);
-        mbar_expect_tx(&kv_full[s], C::kKBytes + C1::kVBytesTma);
-        uint8_t* sk = sKV + s * (C::kKBytes + C::kVBytes);
-        uint8_t* sv = sk + C::kKBytes;
-        for (int dc = 0; dc < C1::kDkChunks; ++dc)
-          tma_load_3d(sk + dc * (BKV * 128), tk, &kv_full[s], dc * 64, head, kvb * nsrc + key0);
-        for (int kc = 0; kc < C1::kKvChunks; ++kc)
-          tma_load_2d(sv + kc * (C::kDV * 128), tv, &kv_full[s], kvb * ldvb + key0 + kc * 64, head * D);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = umma_idesc_f16(kBQ, BKV);
-      constexpr uint32_t idesc_pv = umma_idesc_f16(kBQ, C::kDV);
-      const int n_act = tile_b_active ? 2 : 1;
-      auto issue_qk = [&](int t, int stage) {
-        const uint32_t q_addr = smem_u32(sQ + t * C::kQBytes);
-        const uint32_t k_addr = smem_u32(sKV + stage * (C::kKBytes + C::kVBytes));
-#pragma unroll
-        for (int ks = 0; ks < C1::kKSteps; ++ks) {
-          const int dc = ks >> 2, kk = ks & 3;
-          const uint64_t da = umma_desc_k_sw128(q_addr + dc * (kBQ * 128)) + 2 * kk;
-          const uint64_t db = umma_desc_k_sw128(k_addr + dc * (BKV * 128)) + 2 * kk;
-          umma_f16_ss(tmem_base + t * BKV, da, db, idesc_qk, ks != 0 ? 1u : 0u);
-        }
-        umma_commit(&s_full[t]);
-      };
-      mbar_wait(&q_bar, 0);
-      mbar_wait(&kv_full[0], 0);
-      tc_fence_after_sync();
-      for (int t = 0; t < n_act; ++t) issue_qk(t, 0);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j % C::kStages;
-        const uint32_t v_addr = smem_u32(sKV + s * (C::kKBytes + C::kVBytes)) + C::kKBytes;
-        const bool more = j + 1 < n_tiles;
-        const int s_next = (j + 1) % C::kStages;
-        for (int t = 0; t < n_act; ++t) {
-          // P_t(j) (and the O_t rescale) published by warpgroup t
-          mbar_wait(&p_full[t], j & 1);
-          tc_fence_after_sync();
-          const uint32_t p_addr = smem_u32(sP + t * C::kPBytes);
-#pragma unroll
-          for (int ks = 0; ks < BKV / 16; ++ks) {
-            const int kc = ks >> 2, kk = ks & 3;
-            const uint64_t da = umma_desc_k_sw128(p_addr + kc * (kBQ * 128)) + 2 * kk;
-            const uint64_t db = umma_desc_k_sw128(v_addr + kc * (C::kDV * 128)) + 2 * kk;
-            umma_f16_ss(tmem_base + 2 * BKV + t * C::kDV, da, db, idesc_pv, (j | ks) != 0 ? 1u : 0u);
-          }
-          umma_commit(&o_done[t]);
-          if (t == n_act - 1) umma_commit(&kv_empty[s]);  // every MMA that reads stage s has been issued
-          if (more) {
-            if (t == 0) {
-              mbar_wait(&kv_full[s_next], ((j + 1) / C::kStages) & 1);
-              tc_fence_after_sync();
-            }
-            issue_qk(t, s_next);  // S_t is free: warpgroup t finished reading it before arriving on p_full
-          }
-        }
-      }
-    }
-  } else {
-    // ---------------- softmax warpgroups: warps 2-5 -> Q tile A, warps 6-9 -> Q tile B ----------------
-    const int t = (warp - 2) >> 2;
-    if (t == 0 || tile_b_active) {
-      const int g = warp & 3;
-      const int r = g * 32 + lane;  // query row inside the tile == TMEM lane
-      const uint32_t t_s = tmem_base + (static_cast<uint32_t>(g * 32) << 16) + t * BKV;
-      const uint32_t t_o = tmem_base + (static_cast<uint32_t>(g * 32) << 16) + 2 * BKV + t * C::kDV;
-      float m_run = -INFINITY;
-      float l_run = 0.f;
-      const uint32_t p_row = smem_u32(sP + t * C::kPBytes + (r >> 3) * 1024 + (r & 7) * 128);
-      const int sw = r & 7;
-
-      for (int j = 0; j < n_tiles; ++j) {
-        const bool src1 = j >= t0;
-        const int key0 = (src1 ? (j - t0) : j) * BKV;
-        const int valid = min(BKV, (src1 ? p.n1 : p.n0) - key0);
-        mbar_wait(&s_full[t], j & 1);
-        tc_fence_after_sync();
-        // TMEM reads run at ~64 B/clk/SM, so S (64 KB per 128x128 tile) should be read ONCE.  The exp
-        // reference is therefore chosen before looking at the tile: the running max m_run.  The tile is
-        // exponentiated against it while its own max is tracked; only if some row's max exceeds m_run by
-        // more than 2^8 (first tile, or a rare jump) the warp repeats the pass with the new max.
-        float mt = -INFINITY;
-        float m_new = m_run;
-        float ls0 = 0.f, ls1 = 0.f, ls2 = 0.f, ls3 = 0.f;
-        if (j > 0) {
-          mbar_wait(&o_done[t], (j - 1) & 1);  // PV_t(j-1) done: P_t may be overwritten, O_t rescaled
-          tc_fence_after_sync();
-        }
-        auto pass = [&](bool track_max, bool emit, float neg_m) {
-          uint32_t ra[32], rb[32];
-          tmem_ld_x32(t_s, ra);
-#pragma unroll
-          for (int c = 0; c < BKV / 32; ++c) {
-            uint32_t(&cur)[32] = (c & 1) ? rb : ra;
-            uint32_t(&nxt)[32] = (c & 1) ? ra : rb;
-            tmem_wait_ld();
-            if (c + 1 < BKV / 32) tmem_ld_x32(t_s + (c + 1) * 32, nxt);  // overlaps the math below
-            if (track_max) {
-              if (valid == BKV) {
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) mt = fmax3(mt, __uint_as_float(cur[i]), __uint_as_float(cur[i + 1]));
-              } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i)
-                  if (c * 32 + i < valid) mt = fmaxf(mt, __uint_as_float(cur[i]));
-              }
-            }
-            if (emit) {
-              float pv[32];
-              if (valid == BKV) {  // one FFMA + one MUFU.EX2 + one FADD per element
-#pragma unroll
-                for (int i = 0; i < 32; ++i) pv[i] = ex2_approx(fmaf(__uint_as_float(cur[i]), p.scale_log2, neg_m));
-              } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i)
-                  pv[i] = (c * 32 + i < valid) ? ex2_approx(fmaf(__uint_as_float(cur[i]), p.scale_log2, neg_m)) : 0.f;
-              }
-              if constexpr (!C1::kOnes) {  // (else: the row sum comes out of the PV MMA, O[:, D])
-#pragma unroll
-                for (int i = 0; i < 32; i += 4) {
-                  ls0 += pv[i]; ls1 += pv[i + 1]; ls2 += pv[i + 2]; ls3 += pv[i + 3];
-                }
-              }
-#pragma unroll
-              for (int u4 = 0; u4 < 4; ++u4) {
-                uint4 pk;
-                pk.x = pack_half2(pv[u4 * 8 + 0], pv[u4 * 8 + 1]);
-                pk.y = pack_half2(pv[u4 * 8 + 2], pv[u4 * 8 + 3]);
-                pk.z = pack_half2(pv[u4 * 8 + 4], pv[u4 * 8 + 5]);
-                pk.w = pack_half2(pv[u4 * 8 + 6], pv[u4 * 8 + 7]);
-                const int u = c * 4 + u4;
-                const int kc = u >> 3, uu = u & 7;
-                st_shared_v4(p_row + kc * (kBQ * 128) + ((uu ^ sw) << 4), pk);
-              }
-            }
-          }
-        };
-        bool redo;
-        if (j == 0) {
-          pass(true, false, 0.f);  // no reference yet: max only
-          redo = true;
-        } else {
-          pass(true, true, -m_run);  // optimistic: exponentiate against the running max
-          redo = __any_sync(0xffffffffu, mt * p.scale_log2 - m_run > 8.0f);
-        }
-        if (redo) {
-          const float mts = mt * p.scale_log2;
-          if (mts - m_run > 8.0f) m_new = mts;
-          ls0 = ls1 = ls2 = ls3 = 0.f;
-          pass(false, true, -m_new);
-        }
-        const float alpha = ex2_approx(m_run - m_new);  // m_run = -inf on the first tile -> 0
-        m_run = m_new;
-        if (j > 0 && __any_sync(0xffffffffu, alpha != 1.0f)) {
-#pragma unroll
-          for (int c = 0; c < C::kDV / 16; ++c) {
-            uint32_t oo[16];
-            tmem_ld_x16(t_o + c * 16, oo);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) oo[i] = __float_as_uint(__uint_as_float(oo[i]) * alpha);
-            tmem_st_x16(t_o + c * 16, oo);
-          }
-          tmem_wait_st();
-        }
-        l_run = l_run * alpha + ((ls0 + ls1) + (ls2 + ls3));
-        fence_proxy_async_smem();
-        tc_fence_before_sync();
-        mbar_arrive(&p_full[t]);
-      }
-
-      // final: O / l -> fp16
-      mbar_wait(&o_done[t], (n_tiles - 1) & 1);
-      tc_fence_after_sync();
-      float inv_l = 1.0f / l_run;
-      if constexpr (C1::kOnes) {
-        uint32_t ol[16];
-        tmem_ld_x16(t_o + (D / 16) * 16, ol);
-        tmem_wait_ld();
-        inv_l = 1.0f / __uint_as_float(ol[D % 16]);  // O[:, D] = sum_k P[:, k] (the ones row of V^T)
-      }
-      const int q = q0 + t * kBQ + r;
-      __half* op = p.out + (static_cast<long long>(b) * p.nq + q) * p.ldo + head * D;
-#pragma unroll
-      for (int c = 0; c < C::kDV / 16; ++c) {
-        uint32_t oo[16];
-        tmem_ld_x16(t_o + c * 16, oo);
-        tmem_wait_ld();
-        if (q < p.nq) {
-#pragma unroll
-          for (int h8 = 0; h8 < 2; ++h8) {
-            if (c * 16 + h8 * 8 < D) {
-              uint4 o4;
-              o4.x = pack_half2(__uint_as_float(oo[h8 * 8 + 0]) * inv_l, __uint_as_float(oo[h8 * 8 + 1]) * inv_l);
-              o4.y = pack_half2(__uint_as_float(oo[h8 * 8 + 2]) * inv_l, __uint_as_float(oo[h8 * 8 + 3]) * inv_l);
-              o4.z = pack_half2(__uint_as_float(oo[h8 * 8 + 4]) * inv_l, __uint_as_float(oo[h8 * 8 + 5]) * inv_l);
-              o4.w = pack_half2(__uint_as_float(oo[h8 * 8 + 6]) * inv_l, __uint_as_float(oo[h8 * 8 + 7]) * inv_l);
-              *reinterpret_cast<uint4*>(op + c * 16 + h8 * 8) = o4;
-            }
-          }
-        }
-      }
-    }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, C::kTmemCols);
-  }
-}
-
-void count_launch(int n = 1);
-
-// ------------------------------------------------------------------------------------------------
-// v3: one Q tile per CTA like v1, but the MMA thread runs ONE KEY TILE AHEAD: S is double-buffered in
-// TMEM (S(j+1) = Q K(j+1)^T is computed while the softmax warps work on S(j)), P is double-buffered in
-// shared memory, and the K/V ring is STAGES deep.  The softmax warps therefore never wait for the
-// tensor core (ncu showed ~30% of their stall samples on the s_full barrier in v1/v2); with two CTAs
-// per SM the MUFU pipe — the real bound of d=40 attention — stays fed.
-// TMEM columns: S[0] [0,BKV)  S[1] [BKV,2BKV)  O [2BKV, 2BKV+DV).
-// ------------------------------------------------------------------------------------------------
-template <int D, int BKV, int STAGES>
-struct Attn3Cfg {
-  using C1 = AttnCfg<D, BKV>;
-  static constexpr int kDV = C1::kDV;
-  static constexpr int kQBytes = C1::kQBytes;
-  static constexpr int kKBytes = C1::kKBytes;
-  static constexpr int kVBytes = C1::kVBytes;
-  static constexpr int kPBytes = C1::kPBytes;
-  static constexpr int kSmem = kQBytes + STAGES * (kKBytes + kVBytes) + 2 * kPBytes + 1024;
-  static constexpr int kCols = 2 * BKV + kDV;
-  static constexpr int kTmemCols = kCols <= 128 ? 128 : (kCols <= 256 ? 256 : 512);
-  static constexpr int kCtasPerSm = (kSmem <= 113 * 1024 && kTmemCols <= 256) ? 2 : 1;
-};
-
-template <int D, int BKV, int STAGES, int EMU>  // EMU of every 4 exponentials run on the FMA pipe
-__global__ void __launch_bounds__(kAttnThreads, Attn3Cfg<D, BKV, STAGES>::kCtasPerSm)
-    attn3_tc_kernel(const __grid_constant__ AttnKParams p) {
-  using C = Attn3Cfg<D, BKV, STAGES>;
-  using C1 = AttnCfg<D, BKV>;
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t q_bar;
-  __shared__ __align__(8) uint64_t s_full[2], p_full[2], o_done[2];  // all indexed by tile parity: no barrier
-                                                                       // is ever more than one phase ahead of its waiter
-  __shared__ __align__(8) uint64_t kv_full[STAGES], kv_empty[STAGES];
-  __shared__ uint32_t tmem_base_smem;
-
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
-  uint8_t* sKV = sQ + C::kQBytes;
-  uint8_t* sP = sKV + STAGES * (C::kKBytes + C::kVBytes);  // [2][kPBytes]
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * kBQ;
-  const int head = blockIdx.y;
-  const int b = blockIdx.z;
-  const int t0 = (p.n0 + BKV - 1) / BKV;
-  const int t1 = (b < p.bank_batches && p.n1 > 0) ? (p.n1 + BKV - 1) / BKV : 0;
-  const int n_tiles = t0 + t1;
-
-  pdl_launch_dependents();
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.tmQ);
-    tma_prefetch_desc(&p.tmK0);
-    tma_prefetch_desc(&p.tmV0);
-    mbar_init(&q_bar, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&o_done[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_full[i], 128);
-    }
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, C::kTmemCols);
-  if (warp >= 2)
-    attn_fill_ones_rows<C1, D, STAGES>(sKV, C::kKBytes + C::kVBytes, C::kKBytes, threadIdx.x - 64, kAttnThreads - 64);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_smem;
-  pdl_wait();
-
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(&q_bar, C::kQBytes);
-      for (int dc = 0; dc < C1::kDkChunks; ++dc)
         tma_load_3d(sQ + dc * (kBQ * 128), &p.tmQ, &q_bar, dc * 64, head, b * p.nq + q0);
       for (int j = 0; j < n_tiles; ++j) {
         const int s = j % STAGES;
@@ -731,264 +108,144 @@ __global__ void __launch_bounds__(kAttnThreads, Attn3Cfg<D, BKV, STAGES>::kCtasP
         const int kvb = src1 ? (p.kv1_batches > 1 ? b : 0) : (p.kv0_batches > 1 ? b : 0);
         const int ldvb = src1 ? p.ldv1_batch : p.ldv0_batch;
         mbar_wait(&kv_empty[s], ph ^ 1);
-        mbar_expect_tx(&kv_full[s], C::kKBytes + C1::kVBytesTma);
-        uint8_t* sk = sKV + s * (C::kKBytes + C::kVBytes);
+        mbar_expect_tx(&kv_full[s], C::kStageBytes);
+        uint8_t* sk = sKV + s * C::kStageBytes;
         uint8_t* sv = sk + C::kKBytes;
-        for (int dc = 0; dc < C1::kDkChunks; ++dc)
+        for (int dc = 0; dc < C::kDkChunks; ++dc)
           tma_load_3d(sk + dc * (BKV * 128), tk, &kv_full[s], dc * 64, head, kvb * nsrc + key0);
-        for (int kc = 0; kc < C1::kKvChunks; ++kc)
-          tma_load_2d(sv + kc * (C::kDV * 128), tv, &kv_full[s], kvb * ldvb + key0 + kc * 64, head * D);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = umma_idesc_f16(kBQ, BKV);
-      constexpr uint32_t idesc_pv = umma_idesc_f16(kBQ, C::kDV);
-      const uint32_t q_addr = smem_u32(sQ);
-      auto issue_qk = [&](int j) {  // S[j & 1] = Q K(j)^T
-        const int s = j % STAGES;
-        mbar_wait(&kv_full[s], (j / STAGES) & 1);
-        tc_fence_after_sync();
-        const uint32_t k_addr = smem_u32(sKV + s * (C::kKBytes + C::kVBytes));
-#pragma unroll
-        for (int ks = 0; ks < C1::kKSteps; ++ks) {
-          const int dc = ks >> 2, kk = ks & 3;
-          const uint64_t da = umma_desc_k_sw128(q_addr + dc * (kBQ * 128)) + 2 * kk;
-          const uint64_t db = umma_desc_k_sw128(k_addr + dc * (BKV * 128)) + 2 * kk;
-          umma_f16_ss(tmem_base + (j & 1) * BKV, da, db, idesc_qk, ks != 0 ? 1u : 0u);
-        }
-        umma_commit(&s_full[j & 1]);
-      };
-      mbar_wait(&q_bar, 0);
-      issue_qk(0);
-      for (int j = 0; j < n_tiles; ++j) {
-        // run ahead: S(j+1) while the softmax warps are still on S(j).  Buffer (j+1)&1 was last read for
-        // tile j-1, whose readers finished before arriving on p_full[(j-1)&1] — waited for in iteration j-1.
-        if (j + 1 < n_tiles) issue_qk(j + 1);
-        const int s = j % STAGES;
-        mbar_wait(&p_full[j & 1], (j >> 1) & 1);
-        tc_fence_after_sync();
-        const uint32_t p_addr = smem_u32(sP + (j & 1) * C::kPBytes);
-        const uint32_t v_addr = smem_u32(sKV + s * (C::kKBytes + C::kVBytes)) + C::kKBytes;
-#pragma unroll
-        for (int ks = 0; ks < BKV / 16; ++ks) {
-          const int kc = ks >> 2, kk = ks & 3;
-          const uint64_t da = umma_desc_k_sw128(p_addr + kc * (kBQ * 128)) + 2 * kk;
-          const uint64_t db = umma_desc_k_sw128(v_addr + kc * (C::kDV * 128)) + 2 * kk;
-          umma_f16_ss(tmem_base + 2 * BKV, da, db, idesc_pv, (j | ks) != 0 ? 1u : 0u);
-        }
-        umma_commit(&kv_empty[s]);
-        umma_commit(&o_done[j & 1]);
+        tma_load_2d(sv, tv, &kv_full[s], kvb * ldvb + key0, head * D);
       }
     }
   } else {
-    // ---------------- softmax / correction / epilogue warps ----------------
-    const int g = warp & 3;
-    const int r = g * 32 + lane;
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(g * 32) << 16);
-    const uint32_t t_o = t_lane + 2 * BKV;
-    float m_run = -INFINITY;
-    float l_run = 0.f;
-    const uint32_t p_row0 = smem_u32(sP + (r >> 3) * 1024 + (r & 7) * 128);
-    const int sw = r & 7;
+    // ---------------- warpgroups 0, 1: S, softmax, O ----------------
+    const int wg = warp >> 2;
+    const uint32_t q_addr = smem_u32(sQ) + wg * (64 * 128);  // this warpgroup's 64 query rows of each Q chunk
+    const int cq = 2 * (lane & 3);                           // this thread's first column inside an 8-column block
+    float o[C::kDV / 2];
+#pragma unroll
+    for (int i = 0; i < C::kDV / 2; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY};  // rows r and r + 8 of this thread, log2 domain
+    float l_run[2] = {0.f, 0.f};              // this thread's share of the row sums
+    mbar_wait(&q_bar, 0);
 
     for (int j = 0; j < n_tiles; ++j) {
+      const int s = j % STAGES;
       const bool src1 = j >= t0;
       const int key0 = (src1 ? (j - t0) : j) * BKV;
       const int valid = min(BKV, (src1 ? p.n1 : p.n0) - key0);
-      const uint32_t t_s = t_lane + (j & 1) * BKV;
-      const uint32_t p_row = p_row0 + (j & 1) * C::kPBytes;
-      mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-      tc_fence_after_sync();
-      float mt = -INFINITY;
-      float m_new = m_run;
-      float ls0 = 0.f, ls1 = 0.f, ls2 = 0.f, ls3 = 0.f;
-      // P buffer (j&1) was last read by PV(j-2) — the previous completion of o_done[j&1]
-      if (j >= 2) mbar_wait(&o_done[j & 1], ((j - 2) >> 1) & 1);
-      auto pass = [&](bool track_max, bool emit, float neg_m) {
-        uint32_t ra[32], rb[32];
-        tmem_ld_x32(t_s, ra);
+      mbar_wait(&kv_full[s], (j / STAGES) & 1);
+      const uint32_t k_addr = smem_u32(sKV + s * C::kStageBytes);
+      const uint32_t v_addr = k_addr + C::kKBytes;
+
+      float sc[BKV / 2];
+      wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < BKV / 32; ++c) {
-          uint32_t(&cur)[32] = (c & 1) ? rb : ra;
-          uint32_t(&nxt)[32] = (c & 1) ? ra : rb;
-          tmem_wait_ld();
-          if (c + 1 < BKV / 32) tmem_ld_x32(t_s + (c + 1) * 32, nxt);
-          if (track_max) {
-            if (valid == BKV) {
-#pragma unroll
-              for (int i = 0; i < 32; i += 2) mt = fmax3(mt, __uint_as_float(cur[i]), __uint_as_float(cur[i + 1]));
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (c * 32 + i < valid) mt = fmaxf(mt, __uint_as_float(cur[i]));
-            }
-          }
-          if (emit) {
-            float pv[32];
-            if (valid == BKV) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) {
-                const float xs = fmaf(__uint_as_float(cur[i]), p.scale_log2, neg_m);
-                pv[i] = ((i & 3) < EMU) ? ex2_poly(xs) : ex2_approx(xs);
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                pv[i] = (c * 32 + i < valid) ? ex2_approx(fmaf(__uint_as_float(cur[i]), p.scale_log2, neg_m)) : 0.f;
-            }
-            if constexpr (!C1::kOnes) {  // (else: the row sum comes out of the PV MMA, O[:, D])
-#pragma unroll
-              for (int i = 0; i < 32; i += 4) {
-                ls0 += pv[i]; ls1 += pv[i + 1]; ls2 += pv[i + 2]; ls3 += pv[i + 3];
-              }
-            }
-#pragma unroll
-            for (int u4 = 0; u4 < 4; ++u4) {
-              uint4 pk;
-              pk.x = pack_half2(pv[u4 * 8 + 0], pv[u4 * 8 + 1]);
-              pk.y = pack_half2(pv[u4 * 8 + 2], pv[u4 * 8 + 3]);
-              pk.z = pack_half2(pv[u4 * 8 + 4], pv[u4 * 8 + 5]);
-              pk.w = pack_half2(pv[u4 * 8 + 6], pv[u4 * 8 + 7]);
-              const int u = c * 4 + u4;
-              const int kc = u >> 3, uu = u & 7;
-              st_shared_v4(p_row + kc * (kBQ * 128) + ((uu ^ sw) << 4), pk);
-            }
-          }
-        }
-      };
-      bool redo;
-      if (j == 0) {
-        pass(true, false, 0.f);
-        redo = true;
-      } else {
-        pass(true, true, -m_run);  // optimistic: exponentiate against the running max (S is read once)
-        redo = __any_sync(0xffffffffu, mt * p.scale_log2 - m_run > 8.0f);
+      for (int ks = 0; ks < C::kKSteps; ++ks) {
+        const int dc = ks >> 2, kk = ks & 3;
+        const uint64_t da = wgmma_desc_k_sw128(q_addr + dc * (kBQ * 128)) + 2 * kk;
+        const uint64_t db = wgmma_desc_k_sw128(k_addr + dc * (BKV * 128)) + 2 * kk;
+        wgmma_ss<BKV>(sc, da, db, ks != 0 ? 1u : 0u);
       }
-      if (redo) {
-        const float mts = mt * p.scale_log2;
-        if (mts - m_run > 8.0f) m_new = mts;
-        ls0 = ls1 = ls2 = ls3 = 0.f;
-        pass(false, true, -m_new);
-      }
-      const float alpha = ex2_approx(m_run - m_new);
-      m_run = m_new;
-      if (j > 0 && __any_sync(0xffffffffu, alpha != 1.0f)) {
-        // O must be stable: PV(j-1) complete (rare path — the lazy threshold keeps alpha == 1 almost always)
-        mbar_wait(&o_done[(j - 1) & 1], ((j - 1) >> 1) & 1);
-        tc_fence_after_sync();
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(sc);
+
+      // sc[i]: row r + 8 ((i >> 1) & 1), key 8 (i >> 2) + cq + (i & 1)
+      if (valid < BKV) {
 #pragma unroll
-        for (int c = 0; c < C::kDV / 16; ++c) {
-          uint32_t oo[16];
-          tmem_ld_x16(t_o + c * 16, oo);
-          tmem_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) oo[i] = __float_as_uint(__uint_as_float(oo[i]) * alpha);
-          tmem_st_x16(t_o + c * 16, oo);
-        }
-        tmem_wait_st();
+        for (int i = 0; i < BKV / 2; ++i)
+          if (8 * (i >> 2) + cq + (i & 1) >= valid) sc[i] = -INFINITY;
       }
-      l_run = l_run * alpha + ((ls0 + ls1) + (ls2 + ls3));
-      fence_proxy_async_smem();
-      tc_fence_before_sync();
-      mbar_arrive(&p_full[j & 1]);
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int i = 0; i < BKV / 2; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sc[i]);
+      float alpha[2], neg_m[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+        const float m_new = fmaxf(m_run[h], mx[h] * p.scale_log2);  // a tile holds at least one valid key
+        alpha[h] = ex2_approx(m_run[h] - m_new);                   // m_run = -inf on the first tile -> 0
+        m_run[h] = m_new;
+        neg_m[h] = -m_new;
+      }
+      float ls[2] = {0.f, 0.f};
+      uint32_t pa[BKV / 16][4];
+#pragma unroll
+      for (int i = 0; i < BKV / 2; i += 2) {
+        const int h = (i >> 1) & 1;
+        const float e0 = ex2_approx(fmaf(sc[i], p.scale_log2, neg_m[h]));      // masked keys: exp2(-inf) = 0
+        const float e1 = ex2_approx(fmaf(sc[i + 1], p.scale_log2, neg_m[h]));
+        ls[h] += e0 + e1;
+        pa[i >> 3][(i >> 1) & 3] = pack_half2(e0, e1);  // m16n8k16 A fragment of key slice i / 8
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) l_run[h] = fmaf(l_run[h], alpha[h], ls[h]);
+#pragma unroll
+      for (int i = 0; i < C::kDV / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BKV / 16; ++kk)
+        wgmma_rs<C::kDV>(o, pa[kk], wgmma_desc_k_sw128(v_addr) + 2 * kk, 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+      mbar_arrive(&kv_empty[s]);  // this thread's reads of stage s (through its warpgroup's MMAs) are done
     }
 
-    mbar_wait(&o_done[(n_tiles - 1) & 1], ((n_tiles - 1) >> 1) & 1);
-    tc_fence_after_sync();
-    float inv_l = 1.0f / l_run;
-    if constexpr (C1::kOnes) {
-      uint32_t ol[16];
-      tmem_ld_x16(t_o + (D / 16) * 16, ol);
-      tmem_wait_ld();
-      inv_l = 1.0f / __uint_as_float(ol[D % 16]);  // O[:, D] = sum_k P[:, k] (the ones row of V^T)
-    }
-    const int q = q0 + r;
-    __half* op = p.out + (static_cast<long long>(b) * p.nq + q) * p.ldo + head * D;
+    float inv_l[2];
 #pragma unroll
-    for (int c = 0; c < C::kDV / 16; ++c) {
-      uint32_t oo[16];
-      tmem_ld_x16(t_o + c * 16, oo);
-      tmem_wait_ld();
+    for (int h = 0; h < 2; ++h) {
+      float l = l_run[h];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      inv_l[h] = 1.0f / l;
+    }
+    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int q = q0 + r + 8 * h;
       if (q < p.nq) {
+        __half* op = p.out + (static_cast<long long>(b) * p.nq + q) * p.ldo + head * D + cq;
 #pragma unroll
-        for (int h8 = 0; h8 < 2; ++h8) {
-          if (c * 16 + h8 * 8 < D) {
-            uint4 o4;
-            o4.x = pack_half2(__uint_as_float(oo[h8 * 8 + 0]) * inv_l, __uint_as_float(oo[h8 * 8 + 1]) * inv_l);
-            o4.y = pack_half2(__uint_as_float(oo[h8 * 8 + 2]) * inv_l, __uint_as_float(oo[h8 * 8 + 3]) * inv_l);
-            o4.z = pack_half2(__uint_as_float(oo[h8 * 8 + 4]) * inv_l, __uint_as_float(oo[h8 * 8 + 5]) * inv_l);
-            o4.w = pack_half2(__uint_as_float(oo[h8 * 8 + 6]) * inv_l, __uint_as_float(oo[h8 * 8 + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(op + c * 16 + h8 * 8) = o4;
-          }
-        }
+        for (int c8 = 0; c8 < D / 8; ++c8)
+          *reinterpret_cast<uint32_t*>(op + 8 * c8) =
+              pack_half2(o[4 * c8 + 2 * h] * inv_l[h], o[4 * c8 + 2 * h + 1] * inv_l[h]);
       }
     }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, C::kTmemCols);
   }
 }
 
-template <int D, int BKV, int STAGES, int EMU>
-static int launch_attn3(const AttnKParams& kp, dim3 grid, cudaStream_t st) {
-  using C = Attn3Cfg<D, BKV, STAGES>;
+// d = 40: grids of at least this many 128-row CTAs take the register-capped variant, which runs two CTAs (four MMA
+// warpgroups) per SM; smaller grids keep the uncapped one-CTA-per-SM variant with a deeper ring.  (At d = 80 the
+// capped variant spills: one CTA per SM.)  `scripts/gpu_microbench.py attn` compares the two at self + bank attention
+// of 4096 queries: on an H100 80GB HBM3 (400 W power limit) the capped variant took 335 us against 448 us at 512 CTAs
+// (one frame's cond | uncond batch) and 2.68 ms against 3.68 ms at 4096 (eight frames); grids below 512 CTAs were
+// not measured and keep the uncapped variant.
+// mdb_set_tuning(MDB_TUNE_ATTN40_2Q_MIN_CTAS).
+static int g_attn40_2q_min_ctas = 512;
+int get_attn_tuning() { return g_attn40_2q_min_ctas; }
+void set_attn_tuning(int v) { g_attn40_2q_min_ctas = v; }
+
+template <int D, int BKV, int STAGES, int MINB>
+static int launch_attn(const AttnKParams& kp, dim3 grid, cudaStream_t st) {
+  using C = AttnCfg<D, BKV, STAGES>;
+  static_assert(MINB == 1 || C::kSmem <= 113 * 1024, "two CTAs per SM must fit");
   static bool attr_set = false;
-  auto kern = attn3_tc_kernel<D, BKV, STAGES, EMU>;
+  auto kern = attn_wg_kernel<D, BKV, STAGES, MINB>;
   if (!attr_set) {
     MDB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem));
     attr_set = true;
   }
   MDB_CHECK_CUDA(launch_pdl(kern, grid, dim3(kAttnThreads), C::kSmem, st, kp));
-  count_launch();
-  return MDB_OK;
-}
-
-// d = 40 self-attention (the 64x64 level): grids of at least this many 128-row CTAs go to the two-Q-tile kernel at two
-// CTAs per SM (16 softmax warps per SM).  Measured on B200 (profiles/r02_*): +3.3 % on the eight-frame step (4096
-// CTAs per launch), -2 % on the single-frame step (512 CTAs per launch).  mdb_set_tuning(MDB_TUNE_ATTN40_2Q_MIN_CTAS).
-// d = 80 (the 32x32 level): the one-Q-tile kernel needs 142 KB of shared memory, i.e. ONE CTA and four softmax warps per
-// SM; the two-Q-tile kernel (148 KB, eight softmax warps per SM) takes over at a quarter of the d=40 threshold.
-static int g_attn40_2q_min_ctas = 2048;
-int get_attn_tuning() { return g_attn40_2q_min_ctas; }
-void set_attn_tuning(int v) { g_attn40_2q_min_ctas = v; }
-
-template <int D, int BKV, int MINB = 1>
-static int launch_attn2(const AttnKParams& kp, dim3 grid, cudaStream_t st) {
-  using C = Attn2Cfg<D, BKV>;
-  static_assert(MINB == 1 || (C::kTmemCols <= 256 && C::kSmem <= 113 * 1024), "two CTAs per SM must fit");
-  static bool attr_set = false;
-  auto kern = attn2_tc_kernel<D, BKV, MINB>;
-  if (!attr_set) {
-    MDB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem));
-    attr_set = true;
-  }
-  MDB_CHECK_CUDA(launch_pdl(kern, grid, dim3(kAttn2Threads), C::kSmem, st, kp));
   count_launch();
   return MDB_OK;
 }
 
 template <int D, int BKV>
-static int launch_attn(const AttnKParams& kp, dim3 grid, cudaStream_t st) {
-  using C = AttnCfg<D, BKV>;
-  static bool attr_set = false;
-  auto kern = attn_tc_kernel<D, BKV>;
-  if (!attr_set) {
-    MDB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem));
-    attr_set = true;
-  }
-  MDB_CHECK_CUDA(launch_pdl(kern, grid, dim3(kAttnThreads), C::kSmem, st, kp));
-  count_launch();
-  return MDB_OK;
-}
-
-template <int D, int BKV, int VER>
 static int build_and_launch(const mdb_attn_desc* a, cudaStream_t st) {
-  using C = AttnCfg<D, BKV>;
+  constexpr int kDV = AttnCfg<D, BKV, 1>::kDV;
   AttnKParams kp;
   memset(&kp, 0, sizeof(kp));
   const int hd = a->heads * a->d;
@@ -1006,9 +263,11 @@ static int build_and_launch(const mdb_attn_desc* a, cudaStream_t st) {
     uint32_t box[3] = {64, 1, (uint32_t)BKV};
     int r = make_tmap_f16(tk, k, 3, dims, str, box);
     if (r) return r;
+    // kDV rows from row head * d: rows past d (d = 40 -> 48) are the next head's or zero-filled, and only feed
+    // output columns >= d, which are never stored
     uint64_t vdims[2] = {(uint64_t)nb * ldvb, (uint64_t)hd};
     uint64_t vstr[1] = {(uint64_t)ldvt * 2};
-    uint32_t vbox[2] = {64, (uint32_t)C::kVRowsTma};
+    uint32_t vbox[2] = {64, (uint32_t)kDV};
     return make_tmap_f16(tv, vt, 2, vdims, vstr, vbox);
   };
   if ((rc = mk_kv(a->k0, a->ldk0, a->vt0, a->ldvt0, a->n0, a->kv0_batches, a->ldv0_batch, &kp.tmK0, &kp.tmV0))) return rc;
@@ -1028,26 +287,11 @@ static int build_and_launch(const mdb_attn_desc* a, cudaStream_t st) {
   kp.bank_batches = a->n1 > 0 ? a->bank_batches : 0;
   kp.scale_log2 = a->scale * 1.4426950408889634f;
   dim3 grid((a->nq + kBQ - 1) / kBQ, a->heads, a->batch);
-  if constexpr (VER == 3) {
-    constexpr int ST = (D == 40 ? 4 : 3);
-    if constexpr (D == 40) {
-      // large grids: two Q tiles per CTA AND two CTAs per SM
-      const long long ctas = (long long)grid.x * grid.y * grid.z;
-      if (a->nq > kBQ && ctas >= (long long)g_attn40_2q_min_ctas) {
-        dim3 grid2((a->nq + 2 * kBQ - 1) / (2 * kBQ), a->heads, a->batch);
-        return launch_attn2<D, BKV, 2>(kp, grid2, st);
-      }
-    }
-    if constexpr (D == 80) {
-      const long long ctas = (long long)grid.x * grid.y * grid.z;
-      if (a->nq > kBQ && ctas >= (long long)g_attn40_2q_min_ctas / 4) {
-        dim3 grid2((a->nq + 2 * kBQ - 1) / (2 * kBQ), a->heads, a->batch);
-        return launch_attn2<D, BKV, 1>(kp, grid2, st);
-      }
-    }
-    return launch_attn3<D, BKV, ST, 1>(kp, grid, st);  // 1 of 4 exponentials on the FMA pipe: measured best on B200
+  if constexpr (D == 40) {
+    const long long ctas = (long long)grid.x * grid.y * grid.z;
+    if (ctas >= (long long)g_attn40_2q_min_ctas) return launch_attn<D, BKV, 3, 2>(kp, grid, st);
   }
-  return launch_attn<D, BKV>(kp, grid, st);
+  return launch_attn<D, BKV, (D == 160 ? 2 : 4), 1>(kp, grid, st);
 }
 
 }  // namespace mdb
@@ -1068,11 +312,11 @@ extern "C" int mdb_attention_f16(const mdb_attn_desc* a, mdb_stream_t stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   switch (a->d) {
     case 40:
-      return build_and_launch<40, 64, 3>(a, st);
+      return build_and_launch<40, 64>(a, st);
     case 80:
-      return build_and_launch<80, 64, 3>(a, st);
+      return build_and_launch<80, 64>(a, st);
     case 160:
-      return build_and_launch<160, 64, 1>(a, st);
+      return build_and_launch<160, 64>(a, st);
     default:
       set_error("mdb_attention_f16: head dim %d not supported (40, 80, 160)", a->d);
       return MDB_ERR_UNSUPPORTED;

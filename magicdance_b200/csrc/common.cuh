@@ -1,5 +1,5 @@
-// Shared device/host helpers for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM PTX wrappers,
-// UMMA descriptors, TMA tensor-map construction and error plumbing for the C ABI.
+// Shared device/host helpers for the sm_90a kernels: mbarrier, TMA, cluster and wgmma PTX wrappers,
+// wgmma descriptors, TMA tensor-map construction and error plumbing for the C ABI.
 #pragma once
 
 #include <cuda.h>
@@ -11,6 +11,7 @@
 #include <string.h>
 
 #include "../../include/magicdance_b200.h"
+#include "wgmma.cuh"
 
 namespace mdb {
 
@@ -43,9 +44,6 @@ void set_error(const char* fmt, ...);
 // byte stride of dims[i+1].  Returns 0 on success.
 int make_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                   const uint64_t* strides_bytes, const uint32_t* box);
-// same, un-swizzled (dense row-major box in shared memory): the output map of the TMA-store epilogues
-int make_tmap_f16_plain(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                        const uint64_t* strides_bytes, const uint32_t* box);
 
 // ----------------------------------------------------------------------------------------------
 // device-side PTX wrappers
@@ -67,8 +65,8 @@ inline cudaError_t launch_pdl_cluster2(void (*kernel)(KArgs...), dim3 grid, dim3
   cudaLaunchAttribute attr[2];
   int n = 0;
   if (cluster_z > 1 || cluster_x > 1) {
-    // thread-block cluster: along z = split-K partners reducing through distributed smem,
-    // along x = the CTA pair of a cta_group::2 UMMA (two neighbouring M tiles)
+    // thread-block cluster: along z = split-K partners (GEMM) or the CTAs of one GroupNorm group, which
+    // reduce through distributed shared memory
     attr[n].id = cudaLaunchAttributeClusterDimension;
     attr[n].val.clusterDim.x = cluster_x;
     attr[n].val.clusterDim.y = 1;
@@ -110,8 +108,8 @@ __device__ __forceinline__ bool elect_one() {
 }
 
 // ---- programmatic dependent launch (PDL) ------------------------------------------------------
-// Every kernel of this library (except the persistent gemm_pairp_kernel) starts with pdl_launch_dependents() (the NEXT kernel in the stream may
-// begin its prologue: barrier init, TMEM alloc, descriptor prefetch, index math) and calls pdl_wait()
+// Every kernel of this library starts with pdl_launch_dependents() (the NEXT kernel in the stream may
+// begin its prologue: barrier init, descriptor prefetch, index math) and calls pdl_wait()
 // before it touches global memory (waits until the PREVIOUS kernel has completed and flushed).  With
 // ~650 small kernels per denoise step this was meant to hide launch-to-launch latency (measured: neutral).
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -130,10 +128,6 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// arrive on an mbarrier given as a shared::cluster address (another CTA's barrier, from mapa)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t addr = smem_u32(bar);
@@ -172,40 +166,6 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// CTA-pair (cta_group::2) variants: the destination is THIS CTA's shared memory, the completion bytes are
-// credited to an mbarrier given as a shared::cluster address — the pair leader's `full` barrier.
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                 int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                 int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
-// ---- TMA stores (shared -> global, bulk async-group completion) -----------------------------------
-// The issuing thread's earlier generic-proxy writes of the source tile must be ordered before this with
-// fence_proxy_async_smem() (+ a barrier when other threads wrote parts of the tile).
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// at most N of this thread's bulk groups may still be READING their shared-memory source
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-// all of this thread's bulk groups have completed (writes performed)
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
 // ---- thread-block clusters / distributed shared memory ---------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -232,127 +192,39 @@ __device__ __forceinline__ float4 dsmem_ld_f4(uint32_t cluster_addr) {
 }
 
 // ---- proxies / fences ---------------------------------------------------------------------------
-// generic-proxy smem writes -> visible to the async proxy (tcgen05.mma / TMA reads of smem)
+// generic-proxy smem writes -> visible to the async proxy (wgmma / TMA reads of smem)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// ---- TMEM allocation (one full warp executes these) ---------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// CTA-pair allocation: warp w of BOTH CTAs of the pair executes these (same column range in both SMs)
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ---- UMMA descriptors -----------------------------------------------------------------------------
+// ---- warpgroup MMA (sm_90a) -------------------------------------------------------------------------
 // K-major operand tile stored as [rows][64 halves] (128-byte rows, TMA SWIZZLE_128B, 1024B-aligned):
-// 8-row groups are 1024 B apart (SBO), LBO is ignored for swizzled K-major layouts (set to 1),
-// descriptor version 1 (sm_100), layout type 2 = SWIZZLE_128B.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+// 8-row groups are 1024 B apart (SBO), LBO is unused for swizzled K-major layouts (set to 1),
+// layout type 1 = SWIZZLE_128B.  A K step of 16 halves (32 B) inside the swizzle row is +2 on the descriptor.
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);   // start address  [0,14)
   d |= static_cast<uint64_t>(1) << 16;                      // LBO (unused)   [16,30)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;              // SBO = 1024 B   [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                      // version        [46,48)
-  d |= static_cast<uint64_t>(2) << 61;                      // SWIZZLE_128B   [61,64)
+  d |= static_cast<uint64_t>(1) << 62;                      // SWIZZLE_128B   [62,64)
   return d;
 }
-// kind::f16 instruction descriptor: fp16 A/B (K-major both), fp32 accumulate, shape M x N.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4)                      // c_format = F32
-         | (0u << 7) | (0u << 10)       // a/b format = F16
-         | (0u << 15) | (0u << 16)      // a/b K-major
-         | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+// before the first wgmma of a batch: orders earlier register / shared-memory accesses of the warpgroup
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// at most N committed groups of this warpgroup may still be in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across wgmma_wait
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// named barrier over `threads` threads (a multiple of 32) of this CTA; id 0 is __syncthreads
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
-// commit all prior tcgen05.mma of this thread to an mbarrier (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// CTA-pair UMMA (cta_group::2): D is 256 x N — rows 0..127 in the leader's TMEM, 128..255 in the peer's; each
-// CTA's shared memory holds its own 128 A rows and N/2 of the B rows at the SAME offsets.  Issued by one thread
-// of the leader CTA only.
-__device__ __forceinline__ void umma_f16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit of the leader's prior pair-MMAs: arrives on the mbarrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-
-// same, for a pair that sits at cluster ranks (leader, leader + 1) of a larger cluster
-__device__ __forceinline__ void umma_commit_pair_at(uint64_t* bar, uint32_t leader_rank) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(static_cast<uint16_t>(3u << leader_rank))
-      : "memory");
-}
-
-// ---- TMEM <-> registers (warp w may only touch lanes 32*(w%4) .. +31) -------------------------------
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
@@ -365,49 +237,8 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// exp2 on the FMA/ALU pipes (no MUFU): round-to-nearest split x = n + f with the 1.5*2^23 magic constant,
-// degree-3 polynomial for 2^f on [-0.5, 0.5] (max rel. error 7.7e-5, far below fp16's 4.9e-4), exponent
-// inserted with an integer add.  Attention at head dim 40 is bound by the MUFU pipe; routing a fraction of
-// the exponentials here balances the two pipes (the FlashAttention-4 trick).
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -125.0f);
-  const float t = x + 12582912.0f;
-  const float f = x - (t - 12582912.0f);
-  float p = fmaf(0.05508868f, f, 0.24260405f);
-  p = fmaf(p, f, 0.69327623f);
-  p = fmaf(p, f, 0.99992895f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
-}
-// 3-input max (sm_100+): halves the instruction count of a row-max scan
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)); }
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
-// Exact-GELU with a branch-free polynomial erf (the pair kernel's GEGLU epilogue; case_tuned PAIR): erf(z) ~ z P(z^2) on
-// |z| <= 3 (degree-8 P, weighted least-squares fit on Chebyshev nodes), clamped beyond (1 - erf(3) = 2.2e-5).
-// Max |error| of erf in fp32 Horner arithmetic: 2.1e-5 (scripts/fit_erf_poly.py), i.e. <= 5e-5 absolute on GELU for
-// |x| <= 4.2 — an order of magnitude below the fp16 rounding of the result.  ~16 FMA-pipe instructions, no MUFU, no
-// branches, against ~30 with a divergent branch for erff(): the GEGLU epilogue is bound by exactly this arithmetic.
-__device__ __forceinline__ float gelu_erf_poly_f(float x) {
-  const float z = fminf(fmaxf(x * 0.70710678118654752f, -3.0f), 3.0f);
-  const float u = z * z;
-  float p = 3.912539807232272e-08f;
-  p = fmaf(p, u, -1.883036501622108e-06f);
-  p = fmaf(p, u, 4.0088359475478145e-05f);
-  p = fmaf(p, u, -0.0005029218784834032f);
-  p = fmaf(p, u, 0.004196857435939332f);
-  p = fmaf(p, u, -0.024998900537676144f);
-  p = fmaf(p, u, 0.11093079989966269f);
-  p = fmaf(p, u, -0.3752196488411342f);
-  p = fmaf(p, u, 1.1282506331157733f);
-  const float hx = 0.5f * x;
-  return fmaf(hx, p * z, hx);  // 0.5 x (1 + erf)
-}
-
 #endif  // __CUDACC__
 
 }  // namespace mdb

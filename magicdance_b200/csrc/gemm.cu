@@ -1,20 +1,21 @@
-// tcgen05 GEMM / 3x3 implicit-GEMM convolution for sm_100a.
+// wgmma GEMM / 3x3 implicit-GEMM convolution for sm_90a.
 //
-//   D[M,N] = epilogue(A[M,K] * B[N,K]^T), fp16 operands, fp32 accumulation in TMEM.
+//   D[M,N] = epilogue(A[M,K] * B[N,K]^T), fp16 operands, fp32 accumulation in registers.
 //
 // One CTA computes one 128 x BN output tile (optionally one K-split of it).  Warp roles:
-//   warp 0     TMA producer   — streams 128x64 A tiles and BNx64 B tiles (128B-swizzled) through a
+//   warp 8     TMA producer   — streams 128x64 A tiles and BNx64 B tiles (128B-swizzled) through a
 //                               kStages-deep smem ring; completion on `full` mbarriers.  In conv
 //                               mode the A tile of tap (kh,kw) is a 4-D TMA box over the NHWC
 //                               activation shifted by (kw-1, kh-1): out-of-bounds rows/cols are
 //                               zero-filled by TMA, which IS the pad-1 halo — no im2col buffer.
-//   warp 1     MMA issuer     — one elected lane issues tcgen05.mma (M=128, N=BN, K=16) x4 per
-//                               stage, tcgen05.commit releases the stage (`empty`) and finally
-//                               signals `acc_full`.  Also owns the TMEM allocation.
-//   warps 2-5  epilogue       — tcgen05.ld the accumulator (thread == output row), apply bias /
-//                               per-batch bias (timestep embedding) / residual / GEGLU, store fp16.
-// Two CTAs fit per SM (3 stages, <=108 KB smem, <=256 TMEM columns each) so one CTA's epilogue
-// overlaps the other's main loop.
+//   warps 0-7  two warpgroups, 64 rows each: wgmma (M=64, N=BN, K=16) x4 per stage straight from the
+//                               swizzled smem tiles, one stage in flight while the next is issued; a
+//                               stage is handed back (`empty`) once the MMAs reading it have retired.
+//                               Then the fp32 tile is parked in the idle operand ring and the same
+//                               threads run the epilogue one row per thread: bias / per-batch bias
+//                               (timestep embedding) / residual / GEGLU, fp16 stores.
+// Tiles up to 128 wide with a 3-stage ring fit twice per SM (<= 97 KB smem, <= 112 registers a thread), so one
+// CTA's epilogue overlaps the other's main loop; deep rings and 256-wide tiles run one CTA per SM.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -26,7 +27,9 @@ void set_gemm_tuning(int key, int value);
 
 constexpr int kBM = 128;
 constexpr int kBK = 64;  // 64 halves = 128 B = one swizzle row
-constexpr int kGemmThreads = 192;
+constexpr int kGemmConsumers = 256;                   // warpgroups 0 and 1
+constexpr int kProducerWarp = kGemmConsumers / 32;     // warp 8
+constexpr int kGemmThreads = kGemmConsumers + 32;
 
 struct GemmKParams {
   CUtensorMap tmA;
@@ -56,28 +59,25 @@ struct GemmKParams {
   float ln_eps;
 };
 
-// STAGES = 3: <=108 KB, two CTAs per SM (large grids: the co-resident CTA hides the TMA round trip).
+// STAGES = 3: <=109 KB, two CTAs per SM (large grids: the co-resident CTA hides the TMA round trip).
 // STAGES = 6 (8 for 80-wide tiles): one CTA per SM with a ring deep enough to cover the TMA latency on
 // its own — used when the grid has at most one CTA per SM anyway and the K loop is long.
-// PAIR (gemm_pair_kernel below): two CTAs run ONE cta_group::2 UMMA of shape 256 x BN: each keeps its own
-// 128 A rows and only BN/2 of the B rows, so a 256 x 160 pair tile pulls 26 KB per CTA and K chunk through
-// the L2 -> SM fabric where two independent 128 x 160 tiles pull 36 KB — the fabric (~6.3 KB/clk chip-wide)
-// is what bounds the large GEMMs of this path, not the tensor pipe.
-template <int BN, int STAGES, bool PAIR = false>
+// BN = 256, STAGES = 4 (the large grids, see mdb_gemm_f16): one CTA per SM; half the L2 -> SM bytes per flop of two
+// 128-wide tiles.
+template <int BN, int STAGES>
 struct GemmSmem {
   static constexpr int kABytes = kBM * kBK * 2;
-  static constexpr int kBRows = PAIR ? BN / 2 : BN;
-  static constexpr int kBBytes = kBRows * kBK * 2;
+  static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kTotal = STAGES * kStageBytes + 1024;  // + alignment slack
+  static constexpr int kCtasPerSm = (kTotal <= 113 * 1024 && BN <= 128) ? 2 : 1;
 };
 
 __device__ __forceinline__ void epi_store_chunk(const GemmKParams& p, long long row, int col0, int ncols,
-                                                float (&v)[32], const float* bias_chunk, const uint4* res_pref) {
+                                                float (&v)[32], const float* bias_chunk) {
   // v holds columns col0 .. col0+31 of `row` (fp32 accumulators); bias + residual, then fp16 store.
   // Whole groups of 8 columns go through 16-byte accesses, a ragged tail (N = 77) is scalar.
-  // bias_chunk: this chunk's 32 bias values (shared or global memory) or nullptr;
-  // res_pref:   this chunk's residual, prefetched into registers during the main loop, or nullptr.
+  // bias_chunk: this chunk's 32 bias values (shared or global memory) or nullptr.
   const __half* rp = (p.residual != nullptr) ? p.residual + row * p.ldr + col0 : nullptr;
   __half* dp = p.d + row * p.ldd + col0;
 #pragma unroll
@@ -93,7 +93,7 @@ __device__ __forceinline__ void epi_store_chunk(const GemmKParams& p, long long 
         o[4] += b1.x; o[5] += b1.y; o[6] += b1.z; o[7] += b1.w;
       }
       if (rp != nullptr) {
-        const uint4 r4 = (res_pref != nullptr) ? res_pref[q] : *reinterpret_cast<const uint4*>(rp + q * 8);
+        const uint4 r4 = *reinterpret_cast<const uint4*>(rp + q * 8);
         const __half2* h2 = reinterpret_cast<const __half2*>(&r4);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
@@ -124,16 +124,15 @@ __device__ __forceinline__ void epi_store_chunk(const GemmKParams& p, long long 
 }
 
 template <int BN, bool GEGLU, int kStages>
-__global__ void __launch_bounds__(kGemmThreads, (kStages <= 3) ? 2 : 1)
+__global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPerSm))
     gemm_tc_kernel(const __grid_constant__ GemmKParams p) {
-  using S = GemmSmem<BN, kStages, false>;
+  using S = GemmSmem<BN, kStages>;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kStages];
   __shared__ __align__(8) uint64_t empty_bar[kStages];
-  __shared__ __align__(8) uint64_t acc_bar;
-  __shared__ uint32_t tmem_base_smem;
   __shared__ __align__(16) float s_bias[BN];  // this N tile's bias row (when one row serves all batches)
   __shared__ __align__(16) float s_lnu[BN];   // this N tile's u (LayerNorm folded into the GEMM)
+  __shared__ float2 s_ln[kBM];                // (mean, rstd) of each row of the tile (LayerNorm fusion)
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5;
@@ -144,38 +143,33 @@ __global__ void __launch_bounds__(kGemmThreads, (kStages <= 3) ? 2 : 1)
   const int kc_begin = split * p.chunks_per_split;
   const int kc_end = min(p.k_chunks, kc_begin + p.chunks_per_split);
   const int n_iter = kc_end - kc_begin;
-  constexpr uint32_t kTmemCols = (BN <= 64) ? 64 : (BN <= 128 ? 128 : 256);
-  constexpr int kRedLd = BN + 4;  // fp32 row pitch of the split-K partial tile parked in shared memory
-  static_assert(kBM * kRedLd * 4 <= kStages * S::kStageBytes, "partial tile must fit in the operand ring");
+  constexpr int kRedLd = BN + 4;  // fp32 row pitch of the accumulator tile parked in shared memory
+  static_assert(kBM * kRedLd * 4 <= kStages * S::kStageBytes, "the accumulator tile must fit in the operand ring");
+  const bool ln = p.ln_u != nullptr;
 
   pdl_launch_dependents();
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], p.ln_u != nullptr ? 5 : 1);  // LayerNorm fusion: + one arrival per epilogue warp
+      mbar_init(&empty_bar[s], kGemmConsumers);
     }
-    mbar_init(&acc_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, kTmemCols);
   // a bias row that serves all batches is a constant weight: stage it before the PDL wait (overlaps the
   // previous kernel's tail).  Per-batch biases (timestep embedding) are produced upstream and are read later.
   const bool bias_in_smem = (p.bias != nullptr) && (p.bias_batch_stride == 0) && !p.cluster_reduce;
-  if (bias_in_smem && warp >= 2) {
-    for (int j = threadIdx.x - 64; j < BN; j += 128) s_bias[j] = (n0 + j < p.n) ? p.bias[n0 + j] : 0.f;
+  if (bias_in_smem && warp < kProducerWarp) {
+    for (int j = threadIdx.x; j < BN; j += kGemmConsumers) s_bias[j] = (n0 + j < p.n) ? p.bias[n0 + j] : 0.f;
   }
-  if (p.ln_u != nullptr && warp >= 2) {  // a constant of the weights, like the bias
-    for (int j = threadIdx.x - 64; j < BN; j += 128) s_lnu[j] = (n0 + j < p.n) ? p.ln_u[n0 + j] : 0.f;
+  if (ln && warp < kProducerWarp) {  // a constant of the weights, like the bias
+    for (int j = threadIdx.x; j < BN; j += kGemmConsumers) s_lnu[j] = (n0 + j < p.n) ? p.ln_u[n0 + j] : 0.f;
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_smem;
   pdl_wait();  // everything above overlapped the previous kernel's tail; global memory from here on
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (lane == 0 && n_iter > 0) {
       // conv geometry of this M tile
       int b0 = 0, y0 = 0, x0 = 0;
@@ -205,160 +199,147 @@ __global__ void __launch_bounds__(kGemmThreads, (kStages <= 3) ? 2 : 1)
         tma_load_2d(sb, &p.tmB, &full_bar[s], kc * kBK, n0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && n_iter > 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(kBM, BN);
-      for (int it = 0; it < n_iter; ++it) {
-        const int s = it % kStages;
-        const uint32_t ph = (it / kStages) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after_sync();
-        const uint32_t a_addr = smem_u32(smem + s * S::kStageBytes);
-        const uint32_t b_addr = a_addr + S::kABytes;
-        const uint64_t da = umma_desc_k_sw128(a_addr);
-        const uint64_t db = umma_desc_k_sw128(b_addr);
+  } else {
+    // ---------------- warpgroups 0, 1: main loop on wgmma, then the epilogue ----------------
+    const int wg = warp >> 2;          // this warpgroup's 64 rows of the tile
+    const int tid = threadIdx.x;       // 0 .. kGemmConsumers-1
+    float acc[BN / 2];
 #pragma unroll
-        for (int k = 0; k < kBK / 16; ++k) {
-          // advance 16 halves (32 B) along K inside the 128B swizzle row: +2 in the >>4 address field
-          umma_f16_ss(tmem_base, da + 2 * k, db + 2 * k, idesc, (it | k) != 0 ? 1u : 0u);
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    // LayerNorm folded into the GEMM: statistics of the A rows (pivot-shifted sums, biased variance as nn.LayerNorm),
+    // taken from the A tiles AS THEY PASS THROUGH SHARED MEMORY on their way to the tensor core, while the wgmma of
+    // the stage runs: two threads per row, each summing half of the 64 columns.  No extra global or L2 traffic.
+    const int ln_row = tid >> 1, ln_half = tid & 1;
+    float pivot = 0.f, ls0 = 0.f, ls1 = 0.f, lq0 = 0.f, lq1 = 0.f;
+    for (int it = 0; it < n_iter; ++it) {
+      const int s = it % kStages;
+      mbar_wait(&full_bar[s], (it / kStages) & 1);
+      const uint32_t a_addr = smem_u32(smem + s * S::kStageBytes);
+      const uint64_t da = wgmma_desc_k_sw128(a_addr + wg * (64 * 128));
+      const uint64_t db = wgmma_desc_k_sw128(a_addr + S::kABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBK / 16; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, 1u);
+      wgmma_commit();
+      if (ln) {
+        const uint32_t arow = a_addr + (ln_row >> 3) * 1024 + (ln_row & 7) * 128;
+        if (it == 0) {  // every thread of the row pair takes the row's first element as the pivot
+          uint32_t w0;
+          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w0) : "r"(arow + ((0 ^ (ln_row & 7)) << 4)));
+          pivot = __low2float(*reinterpret_cast<const __half2*>(&w0));
         }
-        umma_commit(&empty_bar[s]);
-      }
-      umma_commit(&acc_bar);
-    }
-  } else if (n_iter > 0) {
-    // ---------------- epilogue warps 2..5 ----------------
-    const int g = warp & 3;  // TMEM lane group this warp may access
-    const long long row = static_cast<long long>(m0) + g * 32 + lane;
-    const bool row_ok = row < p.m;
-    // While the main loop runs these warps are idle: fetch what the epilogue will need — the bias row into
-    // shared memory and this thread's residual row into registers — so that the tail of the kernel does not
-    // pay two dependent global-memory round trips per 32-column chunk.
-    constexpr int kResVecs = (GEGLU ? 0 : ((BN + 31) / 32) * 4);
-    uint4 res_pref[kResVecs > 0 ? kResVecs : 1];
-    const bool res_in_regs = !GEGLU && (p.residual != nullptr) && !p.cluster_reduce && (p.splits == 1);
-    if constexpr (!GEGLU) {
-      if (res_in_regs && row_ok) {
-        const __half* rrow = p.residual + row * p.ldr + n0;
 #pragma unroll
-        for (int q = 0; q < kResVecs; ++q)
-          if (q * 8 + 8 <= BN && n0 + q * 8 + 8 <= p.n) res_pref[q] = *reinterpret_cast<const uint4*>(rrow + q * 8);
-      }
-    }
-    // LayerNorm folded into the GEMM: statistics of this thread's A row (pivot-shifted sums, biased variance as
-    // nn.LayerNorm), taken from the A tiles AS THEY PASS THROUGH SHARED MEMORY on their way to the tensor core — the
-    // epilogue warps are idle during the main loop, wait on the same `full` barriers as the MMA thread and add one
-    // arrival per warp to `empty` (armed with 1 + 4 arrivals in this mode); no extra global or L2 traffic.
-    float ln_mean = 0.f, ln_rstd = 1.f;
-    const bool ln = p.ln_u != nullptr;
-    if (ln) {
-      const int rt = g * 32 + lane;  // row inside the tile == TMEM lane
-      float pivot = 0.f, s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-      for (int it = 0; it < n_iter; ++it) {
-        const int s_ = it % kStages;
-        mbar_wait(&full_bar[s_], (it / kStages) & 1);
-        const uint32_t arow = smem_u32(smem + s_ * S::kStageBytes) + (rt >> 3) * 1024 + (rt & 7) * 128;
-#pragma unroll
-        for (int l = 0; l < 8; ++l) {  // logical 16-byte chunk l lives at physical chunk l ^ (row & 7): conflict-free
+        for (int l = ln_half * 4; l < ln_half * 4 + 4; ++l) {  // logical 16-byte chunk l sits at l ^ (row & 7)
           uint4 u4;
           asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
                        : "=r"(u4.x), "=r"(u4.y), "=r"(u4.z), "=r"(u4.w)
-                       : "r"(arow + ((l ^ (rt & 7)) << 4)));
+                       : "r"(arow + ((l ^ (ln_row & 7)) << 4)));
           const __half2* h2 = reinterpret_cast<const __half2*>(&u4);
-          if (it == 0 && l == 0) pivot = __low2float(h2[0]);
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             const float2 f = __half22float2(h2[e]);
             const float d0 = f.x - pivot, d1 = f.y - pivot;
-            s0 += d0; q0 = fmaf(d0, d0, q0);
-            s1 += d1; q1 = fmaf(d1, d1, q1);
+            ls0 += d0; lq0 = fmaf(d0, d0, lq0);
+            ls1 += d1; lq1 = fmaf(d1, d1, lq1);
           }
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[s_]);  // this warp is done reading stage s_
       }
-      const float inv_k = 1.0f / static_cast<float>(p.k_chunks * kBK);
-      const float ms = (s0 + s1) * inv_k;
-      ln_mean = pivot + ms;
-      ln_rstd = rsqrtf(fmaxf(fmaf(-ms, ms, (q0 + q1) * inv_k), 0.f) + p.ln_eps);
+      wgmma_wait<1>();  // the previous stage's MMAs have finished reading it
+      wgmma_fence_regs(acc);
+      if (it > 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
     }
-    mbar_wait(&acc_bar, 0);
-    tc_fence_after_sync();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(g * 32) << 16);
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if (ln) {
+      float s_ = ls0 + ls1, q_ = lq0 + lq1;
+      s_ += __shfl_xor_sync(0xffffffffu, s_, 1);
+      q_ += __shfl_xor_sync(0xffffffffu, q_, 1);
+      const float inv_k = 1.0f / static_cast<float>(p.k_chunks * kBK);
+      const float ms = s_ * inv_k;
+      if (ln_half == 0) s_ln[ln_row] = make_float2(pivot + ms, rsqrtf(fmaxf(fmaf(-ms, ms, q_ * inv_k), 0.f) + p.ln_eps));
+    }
+    // Both warpgroups' MMAs are complete, so the operand ring is idle: park the fp32 tile in it, [128][kRedLd]
+    // (the layout the split-K cluster reduction reads), and run the epilogue with one thread per row.
+    named_bar_sync(1, kGemmConsumers);
+    float* red = reinterpret_cast<float*>(smem);
+    {
+      const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < BN / 2; j += 2) {
+        const int row_t = r0 + 8 * ((j >> 1) & 1);
+        const int col = 8 * (j >> 2) + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(red + row_t * kRedLd + col) = make_float2(acc[j], acc[j + 1]);
+      }
+    }
+    named_bar_sync(1, kGemmConsumers);
+
+    const int rt = tid & (kBM - 1);   // row inside the tile
+    const int half = tid / kBM;       // which of the tile's column chunks this thread takes (alternating)
+    const long long row = static_cast<long long>(m0) + rt;
+    const bool row_ok = row < p.m;
+    const float* rrow = red + rt * kRedLd;
     if constexpr (!GEGLU) {
+      if (!p.cluster_reduce) {
+        const float2 lnst = ln ? s_ln[rt] : make_float2(0.f, 1.f);
+#pragma unroll 1
+        for (int ch = half; ch < (BN + 31) / 32; ch += 2) {
+          const int col0 = n0 + ch * 32;
+          if (col0 >= p.n) break;
+          float v[32];
 #pragma unroll
-      for (int ch = 0; ch < (BN + 31) / 32; ++ch) {
-        const int col0 = n0 + ch * 32;
-        if (col0 >= p.n) break;  // warp-uniform
-        uint32_t r[32];
-        if (BN % 32 != 0 && ch == BN / 32) {  // 16-column tail of an 80-wide tile
-          uint32_t r16[16];
-          tmem_ld_x16(taddr + ch * 32, r16);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) r[j] = r16[j];
-#pragma unroll
-          for (int j = 16; j < 32; ++j) r[j] = 0u;
-        } else {
-          tmem_ld_x32(taddr + ch * 32, r);
-        }
-        tmem_wait_ld();
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        if (ln) {  // rstd_r (acc - mean_r u[n]); the bias row carries W beta (+ the layer's own bias)
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (ch * 32 + j < BN) v[j] = ln_rstd * fmaf(-ln_mean, s_lnu[ch * 32 + j], v[j]);
-        }
-        const int ncols = min(min(32, BN - ch * 32), p.n - col0);
-        if (p.cluster_reduce) {
-          // split-K inside a cluster: park this CTA's fp32 partial tile in its own shared memory (the
-          // operand ring is idle by now); the cluster reduces it through DSMEM below.
-          float* rp = reinterpret_cast<float*>(smem) + (g * 32 + lane) * kRedLd + ch * 32;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            if (j < ncols) *reinterpret_cast<float4*>(rp + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        } else if (p.splits > 1) {
-          // split-K through global memory: this split's fp32 partial goes to its own workspace slab
-          // (plain vector stores); splitk_finalize_kernel sums the slabs in a fixed order.
-          if (row_ok) {
-            float* wp = p.ws + (static_cast<long long>(split) * p.m + row) * p.n + col0;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              if (j + 4 <= ncols && (p.n & 3) == 0) {
-                *reinterpret_cast<float4*>(wp + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-              } else {
-#pragma unroll
-                for (int e = 0; e < 4; ++e)
-                  if (j + e < ncols) wp[j + e] = v[j + e];
-              }
+          for (int j = 0; j < 32; j += 4) {
+            if (ch * 32 + j < BN) {
+              const float4 f = *reinterpret_cast<const float4*>(rrow + ch * 32 + j);
+              v[j] = f.x; v[j + 1] = f.y; v[j + 2] = f.z; v[j + 3] = f.w;
+            } else {
+              v[j] = v[j + 1] = v[j + 2] = v[j + 3] = 0.f;
             }
           }
-        } else if (row_ok) {
-          const float* bias_chunk = nullptr;
-          if (bias_in_smem) {
-            bias_chunk = s_bias + ch * 32;
-          } else if (p.bias != nullptr) {
-            const long long brow = (p.bias_batch_stride != 0) ? (row / p.rows_per_batch) : 0;
-            bias_chunk = p.bias + brow * p.bias_batch_stride + col0;
+          if (ln) {  // rstd_r (acc - mean_r u[n]); the bias row carries W beta (+ the layer's own bias)
+#pragma unroll
+            for (int j = 0; j < 32; ++j)
+              if (ch * 32 + j < BN) v[j] = lnst.y * fmaf(-lnst.x, s_lnu[ch * 32 + j], v[j]);
           }
-          epi_store_chunk(p, row, col0, ncols, v, bias_chunk, (res_in_regs && ncols == 32) ? &res_pref[ch * 4] : nullptr);
+          const int ncols = min(min(32, BN - ch * 32), p.n - col0);
+          if (p.splits > 1) {
+            // split-K through global memory: this split's fp32 partial goes to its own workspace slab
+            // (plain vector stores); splitk_finalize_kernel sums the slabs in a fixed order.
+            if (row_ok) {
+              float* wp = p.ws + (static_cast<long long>(split) * p.m + row) * p.n + col0;
+#pragma unroll
+              for (int j = 0; j < 32; j += 4) {
+                if (j + 4 <= ncols && (p.n & 3) == 0) {
+                  *reinterpret_cast<float4*>(wp + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+                } else {
+#pragma unroll
+                  for (int e = 0; e < 4; ++e)
+                    if (j + e < ncols) wp[j + e] = v[j + e];
+                }
+              }
+            }
+          } else if (row_ok) {
+            const float* bias_chunk = nullptr;
+            if (bias_in_smem) {
+              bias_chunk = s_bias + ch * 32;
+            } else if (p.bias != nullptr) {
+              const long long brow = (p.bias_batch_stride != 0) ? (row / p.rows_per_batch) : 0;
+              bias_chunk = p.bias + brow * p.bias_batch_stride + col0;
+            }
+            epi_store_chunk(p, row, col0, ncols, v, bias_chunk);
+          }
         }
       }
     } else {
       // GEGLU: chunk pairs (value, gate); output column = n0/2 + pair*32 + j
       const long long brow = (p.bias_batch_stride != 0) ? (row / p.rows_per_batch) : 0;
 #pragma unroll 1
-      for (int pr = 0; pr < BN / 64; ++pr) {
+      for (int pr = half; pr < BN / 64; pr += 2) {
         const int col0 = n0 + pr * 64;
         if (col0 >= p.n) break;
-        uint32_t rv[32], rg[32];
-        tmem_ld_x32(taddr + pr * 64, rv);
-        tmem_ld_x32(taddr + pr * 64 + 32, rg);
-        tmem_wait_ld();
         if (row_ok) {
           const float* bp = bias_in_smem ? (s_bias + pr * 64)
                                          : ((p.bias != nullptr) ? p.bias + brow * p.bias_batch_stride + col0 : nullptr);
+          const float* rv = rrow + pr * 64;
           uint4* d4 = reinterpret_cast<uint4*>(p.d + row * p.ldd + (col0 >> 1));
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
@@ -366,8 +347,8 @@ __global__ void __launch_bounds__(kGemmThreads, (kStages <= 3) ? 2 : 1)
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
               const int j = q * 8 + e;
-              float a = __uint_as_float(rv[j]);
-              float gt = __uint_as_float(rg[j]);
+              float a = rv[j];
+              float gt = rv[32 + j];
               if (bp != nullptr) {
                 a += bp[j];
                 gt += bp[32 + j];
@@ -474,333 +455,6 @@ __global__ void __launch_bounds__(kGemmThreads, (kStages <= 3) ? 2 : 1)
     }
   }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Persistent CTA-pair GEMM (the large grids: eight frames per GPU, the batched appearance passes): one cluster of
-// two CTAs per TPC, ONE CTA per SM (the ~200 KB operand ring keeps every other tensor-memory kernel off the SM),
-// all 512 TMEM columns owned by the pair and used as two accumulator buffers.  Each pair walks the 256 x BN output
-// tiles t = cluster, cluster + #clusters, ... (M fastest, so the pairs running at one time share a B tile); the
-// leader's MMA thread fills buffer (i & 1) for the i-th tile while the epilogue warps of both CTAs drain the other
-// one, and the producers run ahead into the next tile's operands.  Barriers:
-//   full/empty[stage]  both CTAs' TMA bytes are credited to the LEADER's `full`; tcgen05.commit multicast frees a
-//                      stage in both CTAs
-//   acc_full[2]        (each CTA, count 1)   tcgen05.commit multicast: tile i is complete in both CTAs' TMEM
-//   acc_empty[2]       (leader, count 16)    one arrival per epilogue warp of BOTH CTAs: buffer drained
-// Epilogue: EIGHT warps per CTA (two per TMEM lane quarter, each taking half of the tile's 32-column chunks); a warp
-// hands its share of the buffer back as soon as its last tcgen05.ld has returned; the residual of the NEXT chunk
-// is fetched while the current one is converted; output goes through shared memory and TMA (a warp packs 32 rows x
-// 32 columns of fp16 into a 2 KB staging buffer and one lane issues cp.async.bulk.tensor — rows >= M and columns
-// >= N are clipped by the tensor map, whole 64-byte row segments reach L2 instead of 16-byte pieces).
-// Launched WITHOUT programmatic stream serialization and never triggering its dependents early: a pair whose
-// cta_group::2 TMEM allocation is pending must not share its SMs with a foreign tensor-memory CTA (measured: the
-// one-tile-per-launch pair mode of round 1 dead-locked inside the full step for exactly that reason).
-// Measured on B200 (profiles/r02_*): +7 % on the eight-frame step over the single-CTA tiles.
-// ------------------------------------------------------------------------------------------------
-constexpr int kPairqThreads = 320;                    // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
-constexpr int kPairqEpiWarps = 8;
-constexpr int kOutBox = 32;                           // TMA-store box: 32 rows x 32 fp16 columns
-constexpr int kOutBufBytes = kOutBox * kOutBox * 2;   // 2 KB
-
-template <int BN, int STAGES>
-struct PairqSmem {
-  using S = GemmSmem<BN, STAGES, true>;
-  static constexpr int kRing = STAGES * S::kStageBytes;               // multiple of 1024
-  static constexpr int kOut = kPairqEpiWarps * 2 * kOutBufBytes;      // 32 KB
-  static constexpr int kTotal = kRing + kOut + 1024;
-};
-
-// this thread's residual for output columns [col0, col0 + 32) of `row` (N % 8 == 0 is a launch condition)
-__device__ __forceinline__ void pairq_load_res(const GemmKParams& p, long long row, bool row_ok, int col0,
-                                               uint4 (&dst)[4]) {
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    if (row_ok && col0 + q * 8 + 8 <= p.n) dst[q] = *reinterpret_cast<const uint4*>(p.residual + row * p.ldr + col0 + q * 8);
-    else dst[q] = make_uint4(0u, 0u, 0u, 0u);
-  }
-}
-
-template <int BN, bool GEGLU, int kStages>
-__global__ void __launch_bounds__(kPairqThreads, 1)
-    gemm_pair_kernel(const __grid_constant__ GemmKParams p, const __grid_constant__ CUtensorMap tmD) {
-  using S = GemmSmem<BN, kStages, true>;
-  using Q = PairqSmem<BN, kStages>;
-  // UMMA N <= 256: a 320-wide tile (BN = 320, the full width of the 64x64 level: every A tile is loaded exactly once)
-  // is TWO 160-wide MMAs per K step into adjacent accumulator columns.  320 columns leave no room for a second
-  // accumulator buffer, so that tile is single-buffered (the epilogue of a long-K tile is a few % of its main loop).
-  constexpr int kParts = (BN > 256) ? 2 : 1;
-  constexpr int kPartN = BN / kParts;
-  constexpr int kBufs = (BN > 256) ? 1 : 2;
-  static_assert(BN % 32 == 0 && kPartN <= 256 && kPartN % 16 == 0 && BN <= 512, "tile width");
-  static_assert(((kPartN / 2) * 128) % 1024 == 0, "each part's B rows start on a swizzle-atom boundary");
-  static_assert(!GEGLU || BN % 64 == 0, "GEGLU tiles hold (value, gate) chunk pairs");
-  static_assert(Q::kRing % 1024 == 0, "the staging buffers follow the ring and need 128-byte alignment");
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[kStages];
-  __shared__ __align__(8) uint64_t empty_bar[kStages];
-  __shared__ __align__(8) uint64_t acc_full[2];
-  __shared__ __align__(8) uint64_t acc_empty[2];
-  __shared__ uint32_t tmem_base_smem;
-
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  constexpr uint32_t kTmemCols = 512;
-  constexpr uint32_t kAccStride = 256;  // columns between the two accumulator buffers
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.tmA);
-    tma_prefetch_desc(&p.tmB);
-    tma_prefetch_desc(&tmD);
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 2 * kPairqEpiWarps);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_pair(&tmem_base_smem, kTmemCols);
-  tc_fence_before_sync();
-  cluster_sync_all();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_smem;
-  const uint32_t pair_rank = cluster_ctarank();
-  const int n_clusters = gridDim.x >> 1;
-  const int cluster_id = blockIdx.x >> 1;
-  const int m_pairs = (p.m + 2 * kBM - 1) / (2 * kBM);
-  const int n_tiles = (p.n + BN - 1) / BN;
-  const int total_tiles = m_pairs * n_tiles;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t g = 0;  // K chunks issued so far (ring position)
-      for (int t = cluster_id; t < total_tiles; t += n_clusters) {
-        const int mp = t % m_pairs, nt = t / m_pairs;
-        const int m0 = (2 * mp + static_cast<int>(pair_rank)) * kBM;
-        const int n0 = nt * BN;
-        int b0 = 0, y0 = 0, x0 = 0;
-        if (p.conv) {
-          b0 = m0 / p.hw;
-          y0 = (p.hw >= kBM) ? (m0 % p.hw) / p.w : 0;
-          x0 = (p.hw >= kBM) ? (m0 % p.hw) % p.w : 0;
-        }
-        for (int kc = 0; kc < p.k_chunks; ++kc, ++g) {
-          const int s = g % kStages;
-          const uint32_t ph = (g / kStages) & 1;
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          uint8_t* sa = smem + s * S::kStageBytes;
-          uint8_t* sb = sa + S::kABytes;
-          if (pair_rank == 0) mbar_expect_tx(&full_bar[s], 2 * S::kStageBytes);
-          const uint32_t fb = dsmem_map(smem_u32(&full_bar[s]), 0);
-          if (p.conv) {
-            const int tap = kc / p.chunks_per_tap;
-            const int cc = kc - tap * p.chunks_per_tap;
-            const int kh = tap / 3, kw = tap - kh * 3;
-            tma_load_4d_pair(sa, &p.tmA, fb, cc * kBK, p.cs * x0 + kw - 1, p.cs * y0 + kh - 1, b0);
-          } else if (kc < p.k1_chunks) {
-            tma_load_2d_pair(sa, &p.tmA, fb, kc * kBK, m0);
-          } else {
-            tma_load_2d_pair(sa, &p.tmA2, fb, (kc - p.k1_chunks) * kBK, m0);
-          }
-#pragma unroll
-          for (int h = 0; h < kParts; ++h)  // this CTA's half of each part's B rows (tmB's box is kPartN / 2 rows)
-            tma_load_2d_pair(sb + h * (kPartN / 2) * 128, &p.tmB, fb, kc * kBK,
-                             n0 + h * kPartN + static_cast<int>(pair_rank) * (kPartN / 2));
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && pair_rank == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(2 * kBM, kPartN);
-      uint32_t g = 0;
-      int i = 0;
-      for (int t = cluster_id; t < total_tiles; t += n_clusters, ++i) {
-        const int buf = i % kBufs;
-        mbar_wait(&acc_empty[buf], ((i / kBufs) & 1) ^ 1);  // all 16 epilogue warps of the pair have drained this buffer
-        tc_fence_after_sync();
-        const uint32_t tacc = tmem_base + buf * kAccStride;
-        for (int kc = 0; kc < p.k_chunks; ++kc, ++g) {
-          const int s = g % kStages;
-          const uint32_t ph = (g / kStages) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(smem + s * S::kStageBytes);
-          const uint32_t b_addr = a_addr + S::kABytes;
-          const uint64_t da = umma_desc_k_sw128(a_addr);
-          const uint64_t db = umma_desc_k_sw128(b_addr);
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-#pragma unroll
-            for (int h = 0; h < kParts; ++h)
-              umma_f16_ss_pair(tacc + h * kPartN, da + 2 * k, db + h * (((kPartN / 2) * 128) >> 4) + 2 * k, idesc,
-                               (kc | k) != 0 ? 1u : 0u);
-          }
-          umma_commit_pair(&empty_bar[s]);
-        }
-        umma_commit_pair(&acc_full[buf]);
-      }
-    }
-  } else {
-    // ---------------- epilogue warps 2..9 of both CTAs ----------------
-    const int ew = warp - 2;
-    const int gq = warp & 3;     // TMEM lane quarter this warp may access (hardware rule: warp % 4)
-    const int half = ew >> 2;    // which half of the tile's column chunks this warp drains
-    uint8_t* obuf = smem + Q::kRing + ew * (2 * kOutBufBytes);
-    const uint32_t acc_empty_leader0 = dsmem_map(smem_u32(&acc_empty[0]), 0);
-    const uint32_t acc_empty_leader1 = dsmem_map(smem_u32(&acc_empty[1]), 0);
-    constexpr int kUnits = GEGLU ? BN / 64 : BN / 32;   // 32 OUTPUT columns each
-    constexpr int kUnitsLo = (kUnits + 1) / 2;
-    const int u_begin = half ? kUnitsLo : 0;
-    const int u_end = half ? kUnits : kUnitsLo;
-    constexpr int kAccColsPerUnit = GEGLU ? 64 : 32;
-    const bool have_res = !GEGLU && (p.residual != nullptr);
-    uint32_t ob = 0;  // staging-buffer parity, runs on across tiles
-    uint4 rcur[4], rnxt[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) rcur[q] = rnxt[q] = make_uint4(0u, 0u, 0u, 0u);
-    if (have_res && cluster_id < total_tiles) {  // residual of the first tile's first chunk
-      const int mp = cluster_id % m_pairs, nt = cluster_id / m_pairs;
-      const long long row = static_cast<long long>((2 * mp + static_cast<int>(pair_rank)) * kBM) + gq * 32 + lane;
-      pairq_load_res(p, row, row < p.m, nt * BN + u_begin * 32, rcur);
-    }
-    int i = 0;
-    for (int t = cluster_id; t < total_tiles; t += n_clusters, ++i) {
-      const int buf = i % kBufs;
-      const int mp = t % m_pairs, nt = t / m_pairs;
-      const int m0 = (2 * mp + static_cast<int>(pair_rank)) * kBM;
-      const int n0 = nt * BN;
-      const int row0 = m0 + gq * 32;                       // first row of this warp's slab
-      const long long row = static_cast<long long>(row0) + lane;
-      const bool row_ok = row < p.m;
-      const long long brow = (p.bias_batch_stride != 0) ? (row / p.rows_per_batch) : 0;
-      mbar_wait(&acc_full[buf], (i / kBufs) & 1);
-      tc_fence_after_sync();
-      const uint32_t taddr = tmem_base + buf * kAccStride + (static_cast<uint32_t>(gq * 32) << 16);
-      bool arrived = false;
-#pragma unroll 1
-      for (int u = u_begin; u < u_end; ++u) {
-        const int col0 = n0 + u * kAccColsPerUnit;          // first accumulator column of this unit (global N index)
-        if (col0 >= p.n) break;                             // warp-uniform
-        const bool last = (u + 1 == u_end) || (col0 + kAccColsPerUnit >= p.n);
-        uint4 o4[4];
-        if constexpr (!GEGLU) {
-          uint32_t r[32];
-          tmem_ld_x32(taddr + u * 32, r);
-          if (have_res && !last) pairq_load_res(p, row, row_ok, col0 + 32, rnxt);
-          tmem_wait_ld();
-          if (last) {  // this warp's share of the buffer is in registers: hand it back to the MMA thread now
-            tc_fence_before_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(buf == 0 ? acc_empty_leader0 : acc_empty_leader1);
-            arrived = true;
-          }
-          const int ncols = min(32, p.n - col0);
-          const float* bp = (p.bias != nullptr && row_ok) ? p.bias + brow * p.bias_batch_stride + col0 : nullptr;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            float o[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) o[e] = __uint_as_float(r[q * 8 + e]);
-            if (bp != nullptr && q * 8 + 8 <= ncols) {
-              const float4 b0 = *reinterpret_cast<const float4*>(bp + q * 8);
-              const float4 b1 = *reinterpret_cast<const float4*>(bp + q * 8 + 4);
-              o[0] += b0.x; o[1] += b0.y; o[2] += b0.z; o[3] += b0.w;
-              o[4] += b1.x; o[5] += b1.y; o[6] += b1.z; o[7] += b1.w;
-            }
-            if (have_res) {
-              const __half2* h2 = reinterpret_cast<const __half2*>(&rcur[q]);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h2[e]);
-                o[2 * e] += f.x;
-                o[2 * e + 1] += f.y;
-              }
-            }
-            o4[q].x = pack_half2(o[0], o[1]);
-            o4[q].y = pack_half2(o[2], o[3]);
-            o4[q].z = pack_half2(o[4], o[5]);
-            o4[q].w = pack_half2(o[6], o[7]);
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) rcur[q] = rnxt[q];
-        } else {
-          uint32_t rv[32], rg[32];
-          tmem_ld_x32(taddr + u * 64, rv);
-          tmem_ld_x32(taddr + u * 64 + 32, rg);
-          tmem_wait_ld();
-          if (last) {
-            tc_fence_before_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(buf == 0 ? acc_empty_leader0 : acc_empty_leader1);
-            arrived = true;
-          }
-          const float* bp = (p.bias != nullptr && row_ok) ? p.bias + brow * p.bias_batch_stride + col0 : nullptr;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            float o[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const int j = q * 8 + e;
-              float a = __uint_as_float(rv[j]);
-              float gt = __uint_as_float(rg[j]);
-              if (bp != nullptr) {
-                a += bp[j];
-                gt += bp[32 + j];
-              }
-              o[e] = a * gelu_erf_poly_f(gt);
-            }
-            o4[q].x = pack_half2(o[0], o[1]);
-            o4[q].y = pack_half2(o[2], o[3]);
-            o4[q].z = pack_half2(o[4], o[5]);
-            o4[q].w = pack_half2(o[6], o[7]);
-          }
-        }
-        // registers -> staging buffer -> TMA store.  The buffer was last used two stores ago: at most one
-        // younger bulk group may still be reading shared memory.
-        uint8_t* sbuf = obuf + ob * kOutBufBytes;
-        if (lane == 0) tma_store_wait_read<1>();
-        __syncwarp();
-        uint4* srow = reinterpret_cast<uint4*>(sbuf + lane * (kOutBox * 2));
-#pragma unroll
-        for (int q = 0; q < 4; ++q) srow[q] = o4[q];
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0 && row0 < p.m) {
-          tma_store_2d(&tmD, sbuf, GEGLU ? (col0 >> 1) : col0, row0);
-          tma_store_commit();
-        }
-        ob ^= 1u;
-      }
-      if (!arrived) {  // no column of this warp's half lies inside N
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(buf == 0 ? acc_empty_leader0 : acc_empty_leader1);
-      }
-      if (have_res && t + n_clusters < total_tiles) {  // residual of the next tile's first chunk
-        const int tn = t + n_clusters;
-        const int mpn = tn % m_pairs, ntn = tn / m_pairs;
-        const long long rown = static_cast<long long>((2 * mpn + static_cast<int>(pair_rank)) * kBM) + gq * 32 + lane;
-        pairq_load_res(p, rown, rown < p.m, ntn * BN + u_begin * 32, rcur);
-      }
-    }
-    if (lane == 0) tma_store_wait_all();  // the staging buffers must outlive the stores that read them
-  }
-
-  tc_fence_before_sync();
-  cluster_sync_all();  // the leader's MMAs read the partner's shared memory and write its TMEM
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc_pair(tmem_base, kTmemCols);
-  }
 }
 
 // split-K second pass: sum of the fp32 partial slabs ws[splits][M][N] -> bias/residual -> fp16 D
@@ -906,59 +560,26 @@ int make_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* 
   return make_tmap_f16_sw(out, base, rank, dims, strides_bytes, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-int make_tmap_f16_plain(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                        const uint64_t* strides_bytes, const uint32_t* box) {
-  return make_tmap_f16_sw(out, base, rank, dims, strides_bytes, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-}
-
 void count_launch(int n = 1);
 
-// launch heuristics (mdb_set_tuning): defaults selected by the B200 measurements under profiles/
-static int g_pair_min_tiles = 128;  // smallest grid, in 128-row tile equivalents, that goes to gemm_pair_kernel
+// launch heuristics (mdb_set_tuning)
+static int g_pair_min_tiles = 128;  // smallest grid, in 128-row tile equivalents, that goes to the 256-wide tiles
 static int g_bn80_below = 100;      // N % 160 == 0 layers with fewer 160-wide CTAs than this use 80-wide tiles
 constexpr int kLongKChunks = 64;    // ... unless K >= 4096 (automatic split-K): then 160-wide tiles and split K
+constexpr int kSms = 132;           // H100 SXM
 
 template <int BN, bool GEGLU, int STAGES>
 static int launch_gemm(const GemmKParams& kp, dim3 grid, cudaStream_t st) {
   const unsigned cluster_z = kp.cluster_reduce ? static_cast<unsigned>(kp.splits) : 1u;
   static bool attr_set = false;
   auto kern = gemm_tc_kernel<BN, GEGLU, STAGES>;
-  constexpr int kSmem = GemmSmem<BN, STAGES, false>::kTotal;
-  if (!attr_set) {
-    MDB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    attr_set = true;
-  }
-  MDB_CHECK_CUDA(launch_pdl_cluster(kern, grid, dim3(kGemmThreads), kSmem, st, cluster_z, kp));
-  count_launch();
-  return MDB_OK;
-}
-
-template <int BN, bool GEGLU, int STAGES>
-static int launch_gemm_pair(const GemmKParams& kp, const CUtensorMap& tmD, int total_tiles, cudaStream_t st) {
-  static bool attr_set = false;
-  auto kern = gemm_pair_kernel<BN, GEGLU, STAGES>;
-  constexpr int kSmem = PairqSmem<BN, STAGES>::kTotal;
+  constexpr int kSmem = GemmSmem<BN, STAGES>::kTotal;
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
   if (!attr_set) {
     MDB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
     attr_set = true;
   }
-  const int clusters = total_tiles < 74 ? total_tiles : 74;  // one pair per TPC (148 SMs)
-  // no programmatic stream serialization: the pair kernel starts only after its predecessor has completed
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(kPairqThreads);
-  cfg.dynamicSmemBytes = kSmem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  MDB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, kp, tmD));
+  MDB_CHECK_CUDA(launch_pdl_cluster(kern, grid, dim3(kGemmThreads), kSmem, st, cluster_z, kp));
   count_launch();
   return MDB_OK;
 }
@@ -1066,22 +687,20 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
   }
 
   // ---- which kernel ----
-  // Large grids (>= g_pair_min_tiles 128-row tile equivalents, no split-K, at least two M tiles): the persistent
-  // CTA-pair kernel with 256 x {320, 256, 160, 128} tiles — widest first: fewest L2 -> SM bytes per flop; the
-  // 320-wide tile (two 160-wide MMAs per K step, single accumulator buffer) only for long K.
+  // Large grids (>= g_pair_min_tiles 128-row tile equivalents, no split-K, at least two M tiles): 128 x 256 tiles
+  // (N % 256 == 0) or 128 x 160 / 128 x 128 tiles with deep rings, one CTA per SM — widest first: fewest L2 -> SM
+  // bytes per flop.
   const int m_tiles = (g->m + kBM - 1) / kBM;
-  bool pair = g->splits <= 1 && m_tiles >= 2 && g->n % 8 == 0 && g->ln_u == nullptr;  // (the pair kernel has no LN fusion)
+  bool pair = g->splits <= 1 && m_tiles >= 2 && g->n % 8 == 0 && g->ln_u == nullptr;
   int bn = 0;
   if (pair) {
     if (geglu) bn = (g->n % 256 == 0) ? 256 : 0;
-    else if (g->n % 320 == 0 && kp.k_chunks >= 16) bn = 320;
     else if (g->n % 256 == 0) bn = 256;
     else if (g->n % 160 == 0) bn = 160;
     else bn = 128;
-    // ... and enough work per launch: the pair kernel owns its SMs (one ~200 KB CTA each, no PDL, nothing of the other
-    // stream beside it), which only pays when the grid is large AND the K loop is not a handful of chunks
-    // (measured: 8192x320x320 at one frame is faster on the single-CTA tiles, 4096x1280x1280 at eight on the pair)
-    const long long eq = (long long)((m_tiles + 1) / 2) * 2 * ((g->n + bn - 1) / (bn ? bn : 1));
+    // ... and enough work per launch: only a large grid AND a K loop that is not a handful of chunks pays for the
+    // single-CTA-per-SM tiles
+    const long long eq = (long long)m_tiles * ((g->n + bn - 1) / (bn ? bn : 1));
     if (bn == 0 || eq < (long long)g_pair_min_tiles || eq * kp.k_chunks < 16ll * g_pair_min_tiles) pair = false;
   }
   if (pair) {
@@ -1090,18 +709,17 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
     MDB_REQUIRE(g->n % 128 == 0, "mdb_gemm_f16: GEGLU needs N %% 128 == 0 (N=%d)", g->n);
     bn = 128;
   } else if (g->n % 160 == 0) {
-    // 160-wide tiles unless that leaves most of the 148 SMs idle; then (short K) halve the tile width, or (long K:
+    // 160-wide tiles unless that leaves most of the SMs idle; then (short K) halve the tile width, or (long K:
     // the weight-streaming 3x3 convs of the 8x8 ... 32x32 levels at one frame) keep the wide tile and split K —
-    // see auto_splits below and profiles/r02_deepk_microbench.md
+    // see the automatic split-K below (scripts/gpu_microbench.py times the tile width x split-K choices)
     const long long tiles160 = (long long)m_tiles * (g->n / 160) * (g->splits > 1 ? g->splits : 1);
-    const bool wide_split = g->splits == 0 && kp.k_chunks >= kLongKChunks && tiles160 * 2 <= 148;
+    const bool wide_split = g->splits == 0 && kp.k_chunks >= kLongKChunks && tiles160 * 2 <= kSms;
     bn = (tiles160 < g_bn80_below && !wide_split) ? 80 : 160;
   } else {
     bn = 128;
   }
   {
-    // a pair CTA stages half of the B rows (of each 160-wide part of a 320-wide tile)
-    uint32_t box[2] = {kBK, (uint32_t)(pair ? (bn == 320 ? 80 : bn / 2) : bn)};
+    uint32_t box[2] = {kBK, (uint32_t)bn};
     uint64_t dims[2] = {(uint64_t)g->k, (uint64_t)g->n};
     uint64_t str[1] = {(uint64_t)g->ldb * 2};
     rc = make_tmap_f16(&kp.tmB, g->b, 2, dims, str, box);
@@ -1112,12 +730,12 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
   if (g->ln_u != nullptr) splits = 1;  // the correction is applied by the CTA that holds the whole K range
   if (g->splits == 0 && !geglu && !pair && g->ln_u == nullptr) {
     // automatic split-K: a power of two up to 8 (reduced inside a thread-block cluster through DSMEM) that brings
-    // the grid to about one CTA per SM while every split keeps at least 16 K chunks (measured on B200 with cold
-    // weights: below that the cluster reduction costs more than the extra CTAs gain)
+    // the grid to about one CTA per SM while every split keeps at least 16 K chunks (below that the cluster
+    // reduction costs more than the extra CTAs gain)
     const long long tiles = (long long)m_tiles * ((g->n + bn - 1) / bn);
     if (tiles < 100)
       for (int c = 8; c >= 2; c >>= 1)
-        if (tiles * c <= 148 && kp.k_chunks / c >= 16) {
+        if (tiles * c <= kSms && kp.k_chunks / c >= 16) {
           splits = c;
           break;
         }
@@ -1136,21 +754,12 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
   }
 
   dim3 grid(m_tiles, (g->n + bn - 1) / bn, splits);
-  const bool deep = (long long)grid.x * grid.y * grid.z <= 148 && kp.chunks_per_split >= 12;
+  const bool deep = (long long)grid.x * grid.y * grid.z <= kSms && kp.chunks_per_split >= 12;
   if (pair) {
-    // output tensor map of the TMA-store epilogue: [M][N_out] fp16, 32 x 32 boxes, dense (no swizzle)
-    CUtensorMap tmD;
-    uint32_t boxd[2] = {(uint32_t)kOutBox, (uint32_t)kOutBox};
-    uint64_t dimsd[2] = {(uint64_t)(geglu ? g->n / 2 : g->n), (uint64_t)g->m};
-    uint64_t strd[1] = {(uint64_t)g->ldd * 2};
-    rc = make_tmap_f16_plain(&tmD, g->d, 2, dimsd, strd, boxd);
-    if (rc) return rc;
-    const int total_tiles = ((m_tiles + 1) / 2) * (int)grid.y;
-    if (geglu) return launch_gemm_pair<256, true, 5>(kp, tmD, total_tiles, st);
-    if (bn == 320) return launch_gemm_pair<320, false, 5>(kp, tmD, total_tiles, st);
-    if (bn == 160) return launch_gemm_pair<160, false, 6>(kp, tmD, total_tiles, st);
-    if (bn == 256) return launch_gemm_pair<256, false, 5>(kp, tmD, total_tiles, st);
-    return launch_gemm_pair<128, false, 6>(kp, tmD, total_tiles, st);
+    if (bn == 256) rc = geglu ? launch_gemm<256, true, 4>(kp, grid, st) : launch_gemm<256, false, 4>(kp, grid, st);
+    else if (bn == 160) rc = launch_gemm<160, false, 6>(kp, grid, st);
+    else rc = launch_gemm<128, false, 6>(kp, grid, st);
+    return rc;
   }
   if (geglu) rc = launch_gemm<128, true, 3>(kp, grid, st);
   else if (bn == 160) rc = deep ? launch_gemm<160, false, 6>(kp, grid, st) : launch_gemm<160, false, 3>(kp, grid, st);
@@ -1160,7 +769,7 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
   if (splits > 1 && !kp.cluster_reduce) {
     const long long total = ((long long)g->m * g->n + 3) / 4;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > kSms * 8) blocks = kSms * 8;
     MDB_CHECK_CUDA(launch_pdl(splitk_finalize_kernel, dim3(blocks), dim3(256), 0, st, kp));
     count_launch();
   }

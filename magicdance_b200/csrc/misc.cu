@@ -110,10 +110,13 @@ __global__ void __launch_bounds__(256) direct_conv3x3_kernel(const __half* __res
 // ---------------------------------------------------------------------------------------------
 constexpr int kCiSlots = 8;
 constexpr int kCiPixPerThread = 4;
+constexpr int kCiMaxThreads = 512;
+// Blocks of kCiSlots * (cout / 8) <= kCiMaxThreads threads: the register budget must admit the largest.
 template <int CIN>
-__global__ void conv3x3_smallcin_kernel(const __half* __restrict__ x, const __half* __restrict__ wt,
-                                        const float* __restrict__ bias, const __half* __restrict__ residual,
-                                        __half* __restrict__ y, int batch, int h, int w, int cout, int silu) {
+__global__ void __launch_bounds__(kCiMaxThreads) conv3x3_smallcin_kernel(const __half* __restrict__ x, const __half* __restrict__ wt,
+                                                                const float* __restrict__ bias, const __half* __restrict__ residual,
+                                                                __half* __restrict__ y, int batch, int h, int w, int cout,
+                                                                int silu) {
   extern __shared__ float s_wt[];  // [9*CIN][8][groups]
   constexpr int KK = 9 * CIN;
   const int groups = cout / 8;
@@ -452,7 +455,7 @@ __global__ void cfg_ddim_update_kernel(float* x, const float* __restrict__ ec, c
 }
 
 
-static inline int grid_for(long long total, int threads = 256, int cap = 148 * 16) {
+static inline int grid_for(long long total, int threads = 256, int cap = 132 * 16) {
   long long b = (total + threads - 1) / threads;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
@@ -503,8 +506,8 @@ extern "C" int mdb_device_check(void) {
   MDB_CHECK_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   MDB_CHECK_CUDA(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) {
-    set_error("device %d is sm_%d%d; this library is built for sm_100a only", dev, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device %d is sm_%d%d; this library is built for sm_90a only", dev, prop.major, prop.minor);
     return MDB_ERR_UNSUPPORTED;
   }
   return MDB_OK;
@@ -597,7 +600,7 @@ extern "C" int mdb_conv3x3_direct_f16(const void* x, const void* wt, const float
   dim3 grid(((wo + kDcTile - 1) / kDcTile) * ((ho + kDcTile - 1) / kDcTile), (cout + kDcCout - 1) / kDcCout, batch);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long npix = static_cast<long long>(batch) * h * w;
-  if (stride == 1 && cin == 4 && cout % 8 == 0 && cout * 36 * 4 <= 96 * 1024 && kCiSlots * (cout / 8) <= 1024) {
+  if (stride == 1 && cin == 4 && cout % 8 == 0 && cout * 36 * 4 <= 96 * 1024 && kCiSlots * (cout / 8) <= kCiMaxThreads) {
     // tiny-cin path (input conv)
     static bool attr_set = false;
     const int smem = cout * 36 * 4;
@@ -623,7 +626,7 @@ extern "C" int mdb_conv3x3_direct_f16(const void* x, const void* wt, const float
       attr_set = true;
     }
     int blocks = static_cast<int>((npix + 7) / 8);
-    if (blocks > 148 * 4) blocks = 148 * 4;
+    if (blocks > 132 * 4) blocks = 132 * 4;
     MDB_CHECK_CUDA(launch_pdl(conv3x3_smallcout_kernel<4>, dim3(blocks), dim3(256), smem, st,
                               static_cast<const __half*>(x), static_cast<const __half*>(wt), bias,
                               static_cast<__half*>(y), batch, h, w, cin, silu));

@@ -376,10 +376,10 @@ extern "C" int64_t mdb_groupnorm_ws_floats(int32_t c, int32_t batch, int32_t hw)
   return kGnMaxBatch + static_cast<int64_t>(batch) * 64 + static_cast<int64_t>(batch) * nblk * 64;
 }
 
-// single-launch cluster path: needs even channels per group.  Automatic choice (measured on B200, scripts/gpu_microbench.py
-// gn -> profiles/r02_gn_microbench.md): the cluster kernel wins at every batch size once a group is >= 20 channels wide
-// (>= 40 bytes per pixel: whole sectors); with 10-channel groups (the 320-channel layers of the 64x64 level) its 20-byte
-// slivers waste half of every sector and it only wins while the launch count dominates (batch <= 2).
+// single-launch cluster path: needs even channels per group.  Automatic choice (scripts/gpu_microbench.py gn compares
+// the two paths): the cluster kernel is taken once a group is >= 20 channels wide (>= 40 bytes per pixel: whole
+// sectors); with 10-channel groups (the 320-channel layers of the 64x64 level) its 20-byte slivers waste half of every
+// sector, so it is taken only while the launch count dominates (batch <= 2).
 // mode: 0 = automatic, 1 = force the two-kernel path, 2 = force the cluster path (tests)
 static bool gn_use_cluster(int c, int c1, int c2, int batch, int mode) {
   const bool ok = (c % 64 == 0) && (c1 % 2 == 0) && (c2 % 2 == 0) && (c / 64 <= kGnFusedThreads);
@@ -399,7 +399,7 @@ extern "C" int mdb_groupnorm_f16(const void* x1, int32_t c1, const void* x2, int
   if (gn_use_cluster(c, c1, c2, batch, mode)) {
     // cluster size: enough CTAs to cover the SMs about twice, at least ~64 pixels per CTA, at most 8 (portable)
     int cs = 1;
-    while (cs < 8 && 32 * batch * cs * 2 <= 320 && hw / (cs * 2) >= 64) cs *= 2;
+    while (cs < 8 && 32 * batch * cs * 2 <= 2 * 132 && hw / (cs * 2) >= 64) cs *= 2;  // 132 SMs
     MDB_CHECK_CUDA(launch_pdl_cluster(gn_cluster_kernel, dim3(32, batch, cs), dim3(kGnFusedThreads), 0, st,
                                       static_cast<unsigned>(cs), static_cast<const __half*>(x1), c1,
                                       static_cast<const __half*>(x2), c2, gamma, beta, static_cast<__half*>(y), hw, eps,

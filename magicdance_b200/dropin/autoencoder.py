@@ -4,8 +4,8 @@ same constructor kwargs, the same 248 state-dict keys and shapes (`encoder.*`, `
 `encode(x) -> posterior` / `decode(z) -> image` / `forward(input, sample_posterior)` calls — running on the hot
 path's kernels through magicdance_b200/vae.py.
 
-Validated on a B200 against the goldens of the unmodified reference AutoencoderKL (tests/test_vae_gpu.py: decode
-and encode rel-L2 ~1.5e-3 at fp16 storage) and re-exported under the reference's dotted path
+Checked against the goldens of the unmodified reference AutoencoderKL (tests/test_vae_gpu.py: decode and encode
+within rel-L2 5e-3 at fp16 storage) and re-exported under the reference's dotted path
 `model_lib/ControlNet/ldm/models/autoencoder.py`, so the YAML's first_stage_config resolves to it.
 Parameters stay fp32 in PyTorch-native layouts (checkpoint compatible); the fp16 kernel layouts are packed lazily on
 the GPU and dropped by load_state_dict.  Inference only: no loss, no EMA, no training_step.

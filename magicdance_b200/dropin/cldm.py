@@ -8,7 +8,7 @@
 Same constructor kwargs (models/cldm_v15_reference_only_pose.yaml), same forward / apply_model
 signatures, same state-dict keys.  Tensors cross this boundary exactly as in the reference (NCHW fp32
 latents, (B,77,768) context, lists of tensors for the bank and the pose residuals); inside, everything
-runs on the sm_100a kernels in fp16 channels-last.
+runs on the sm_90a kernels in fp16 channels-last.
 """
 from __future__ import annotations
 

@@ -4,7 +4,7 @@ for the configuration the MagicPose scripts drive (test_tiktok.py:261-268): eps-
 classifier-free guidance through the 'controlnet is more important' branch (ddim.py:598-605).
 
 Host code only: the step itself (pose ControlNet, paired conditional/unconditional UNet, fused
-CFG + DDIM update) runs on the sm_100a kernels via magicdance_b200.pipeline.DenoisePipeline, which also
+CFG + DDIM update) runs on the sm_90a kernels via magicdance_b200.pipeline.DenoisePipeline, which also
 keeps the per-sequence caches (text K/V, per-timestep appearance bank, per-frame hint features) across
 the frames of a video — the reference recomputes all of them for every frame and step.
 """

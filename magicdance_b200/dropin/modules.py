@@ -1,7 +1,7 @@
 """Parameter-holding nn.Module tree with the reference's class names, constructor kwargs and
 state-dict keys (SURVEY §8b) for the three networks of the hot path.  The modules own fp32
 parameters exactly like the reference's (Conv2d OIHW, Linear (out,in)); their forward()s do not run
-PyTorch operators — they hand the tensors to the sm_100a engine (magicdance_b200.engine).
+PyTorch operators — they hand the tensors to the sm_90a engine (magicdance_b200.engine).
 
 Reference layout being mirrored (paths relative to model_lib/ControlNet/):
   ResBlock / Upsample / Downsample / TimestepEmbedSequential / UNetModel

@@ -1,4 +1,4 @@
-"""Host-side schedule of the denoising hot path over the sm_100a kernels (magicdance_b200.ops).
+"""Host-side schedule of the denoising hot path over the sm_90a kernels (magicdance_b200.ops).
 
 Implements, for the reference's three networks and their glue:
   ControlledUnetModelAttnPose.forward   model_lib/ControlNet/cldm/cldm.py:59-112

@@ -57,9 +57,9 @@ def _chk(t: torch.Tensor, dtype, name):
 
 
 def require_cuda(device):
-    """The single place that decides where the networks may live: an sm_100 CUDA device, nothing else."""
+    """The single place that decides where the networks may live: an sm_90 CUDA device, nothing else."""
     if torch.device(device).type != "cuda":
-        raise RuntimeError("magicdance_b200: the networks run only on an sm_100 CUDA device — move the model to "
+        raise RuntimeError("magicdance_b200: the networks run only on an sm_90 CUDA device — move the model to "
                            "the GPU first (there is no CPU/PyTorch fallback for the hot path)")
 
 

@@ -1,4 +1,4 @@
-"""DDIM step scheduler over the DenoiseEngine: the B200-side counterpart of
+"""DDIM step scheduler over the DenoiseEngine: the GPU-side counterpart of
 DDIMSampler_ReferenceOnly (model_lib/ControlNet/ldm/models/diffusion/ddim.py:346-730), restricted
 to the path MagicPose's inference script drives (test_tiktok.py:261-268): eps-parameterisation,
 'controlnet is more important' CFG branch (ddim.py:598-605), wonoise=True (ddim.py:532-533).
@@ -217,7 +217,7 @@ class GraphedDenoiser:
     def _step_body(self):
         """One DDIM step.  The pose ControlNet and the UNet's encoder half are independent (the pose
         residuals enter at the middle block, cldm.py:93-104), and at one frame per GPU each of their
-        kernels fills only part of the 148 SMs, so the ControlNet runs on a second stream (forked and
+        kernels fills only part of the 132 SMs, so the ControlNet runs on a second stream (forked and
         joined with events, captured into the same graph) with its own scratch buffers."""
         eng, b = self.eng, self.batch
         prev_aux, eng.aux_streams = eng.aux_streams, self.aux_streams

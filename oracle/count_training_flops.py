@@ -6,7 +6,7 @@ CrossAttention inside backward, util.py:118-187) and once without.
 
 Run in the build container only (needs /root/reference):
 
-    cd /tmp && python /root/repo/oracle/count_training_flops.py      # writes profiles/r02_training_flops.md
+    python oracle/count_training_flops.py      # writes profiles/r02_training_flops.md
 """
 from __future__ import annotations
 

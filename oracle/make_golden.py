@@ -162,7 +162,6 @@ def main():
     print(f"[full64] reference p_sample_ddim {dt:.1f}s on {torch.get_num_threads()} threads", flush=True)
     _put(store, "full64/x_prev", x_prev, whole=True)
     _put(store, "full64/pred_x0", pred_x0, whole=True)
-    store["full64/p_sample_seconds"] = np.asarray(dt)
     store["full64/ddim_timesteps"] = np.asarray(sampler.ddim_timesteps)
     store["full64/ddim_alphas"] = np.asarray(sampler.ddim_alphas, dtype=np.float64)
     store["full64/ddim_alphas_prev"] = np.asarray(sampler.ddim_alphas_prev, dtype=np.float64)
@@ -172,6 +171,10 @@ def main():
     a_t = float(sampler.ddim_alphas[index])
     chk = (inp["x"] - float(np.sqrt(1 - a_t)) * e_t) / a_t ** 0.5
     print("pred_x0 self-consistency max abs:", float((chk - pred_x0).abs().max()))
+    # the per-layer summaries (bank / pose / tap) stay out of full64.npz — small32.npz carries them and the file must
+    # stay under 1 MB; what the tests read is the step's outputs and the schedule
+    store = {k: v for k, v in store.items() if k.startswith(("full64/eps_", "full64/x_prev", "full64/pred_x0",
+                                                             "full64/ddim_", "full64/alphas_cumprod"))}
     np.savez_compressed(os.path.join(GOLDEN, "full64.npz"), **store)
     print("golden written to", GOLDEN)
 

@@ -97,7 +97,7 @@ def main():
         conv_case(2, 8, 8, 2560, 1280, 16)
         conv_case(8, 8, 8, 1280, 1280, 4)
     if which == "pair":
-        # single-CTA 128 x BN tiles vs the persistent CTA-pair kernel (256 x BN, cta_group::2), shape by shape, at the cond+uncond batch of one frame (2) and of eight frames (16)
+        # two-CTA-per-SM 128 x BN tiles vs the one-CTA-per-SM large-grid tiles (128 x 256 / deep rings), shape by shape, at the cond+uncond batch of one frame (2) and of eight frames (16)
         big = 1 << 30
         for label, tune in (("single-CTA tiles", dict(pair_min_tiles=big)), ("pair kernel (forced)", dict(pair_min_tiles=1))):
             print(f"--- {label}", flush=True)
@@ -135,7 +135,7 @@ def main():
         return
     if which == "deepk":
         # the single-frame weight-streaming layers (cond+uncond batch of 2) with COLD weights, as inside a step (each
-        # step streams 2.4 GB of weights through a 126 MB L2): eight weight copies are cycled; 80- vs 160-wide tiles
+        # step streams 2.4 GB of weights through a 50 MB L2): eight weight copies are cycled; 80- vs 160-wide tiles
         # and the split-K factor
         def cold(name, m, n, k, conv, flops):
             ws = [h(n, k) for _ in range(max(2, int(300e6 / (2.0 * n * k)) + 1))]
@@ -161,14 +161,15 @@ def main():
             cold(f"gemm m={m} n={n} k={k}", m, n, k, None, 2.0 * m * n * k)
         return
     if which in ("all", "attn"):
-        attn_case(1, 40, 4096, 4096)
-        attn_case(1, 40, 4096, 4096, 4096)
-        attn_case(8, 40, 4096, 4096, 4096)
+        # d=40 (the 64x64 level, self tokens + bank): the register-capped two-CTA-per-SM variant (key 0) against the
+        # one-CTA-per-SM variant (key 2^30) at the cond|uncond batch of one frame (512 CTAs) and of eight (4096 CTAs)
+        for b in (2, 16):
+            for key in (0, 1 << 30):
+                with ops.tuning(attn40_2q_min_ctas=key):
+                    print(f"attn40_2q_min_ctas={key}:", end=" ", flush=True)
+                    attn_case(b, 40, 4096, 4096, 4096)
         attn_case(1, 40, 4096, 77)
         attn_case(16, 80, 1024, 1024, 1024)
-        with ops.tuning(attn40_2q_min_ctas=1 << 30):
-            attn_case(16, 80, 1024, 1024, 1024)   # one-Q-tile kernel for comparison
-            attn_case(8, 40, 4096, 4096, 4096)
         attn_case(1, 80, 1024, 1024, 1024)
         attn_case(1, 80, 1024, 77)
         attn_case(1, 160, 256, 256, 256)

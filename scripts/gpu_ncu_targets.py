@@ -39,7 +39,7 @@ for _ in range(reps):
         ops.groupnorm(x1, g_, b_, batch=b, hw=hw, eps=1e-5, silu=True, x2=x2)
     x, g_, b_ = h(8192, 320), f(320), f(320)
     ops.layernorm(x, g_, b_)
-    # ---- eight frames per GPU (cond | uncond batch of 16): the persistent CTA-pair GEMM, the two-Q-tile attention,
+    # ---- eight frames per GPU (cond | uncond batch of 16): the large-grid GEMM tiles, the two-CTA-per-SM d=40 attention,
     # the two-kernel GroupNorm ----
     for (b, hh, cin, cout) in ((16, 32, 1280, 640), (16, 16, 1280, 1280), (16, 64, 320, 320)):
         x, w, bias = h(b * hh * hh, cin), h(cout, 9 * cin), f(cout)

@@ -1,6 +1,6 @@
 """profiles/traffic.json from the ncu launch lists of one captured DDIM step (NVTX-scoped: `bench.py --nvtx` under
 `ncu --nvtx --nvtx-include "mdb_step/"` with dram__bytes_read.sum / dram__bytes_write.sum / gpu__time_duration.sum):
-per frames-per-GPU, the DRAM bytes and time of the tcgen05 GEMM family (gemm_tc_kernel + gemm_pair_kernel) and of attention.
+per frames-per-GPU, the DRAM bytes and time of the wgmma GEMM (gemm_tc_kernel) and of attention.
 
     python scripts/ncu_traffic.py profiles/traffic.json 1=gpurun_out/launches_b1.csv 8=gpurun_out/launches_b8.csv
 """
@@ -24,7 +24,7 @@ def one(path, frames):
     ends = [i for i, l in enumerate(launches) if "cfg_ddim_update" in l["name"]]
     step = launches[ends[-2] + 1: ends[-1] + 1] if len(ends) >= 2 else launches
     out = {}
-    for key, pats in (("gemm_tc_kernel_b%d" % frames, ("gemm_tc_kernel", "gemm_pair_kernel")), ("attention_b%d" % frames, ("attn",))):
+    for key, pats in (("gemm_tc_kernel_b%d" % frames, ("gemm_tc_kernel",)), ("attention_b%d" % frames, ("attn",))):
         sel = [l for l in step if any(p in l["name"] for p in pats)]
         rd = sum(l.get("dram__bytes_read.sum", 0) for l in sel)
         wr = sum(l.get("dram__bytes_write.sum", 0) for l in sel)

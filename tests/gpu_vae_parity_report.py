@@ -1,5 +1,5 @@
 """GPU parity of the VAE decoder and encoder in magicdance_b200/vae.py against the pinned CPU oracle and
-the reference goldens.  Run on a B200:
+the reference goldens.  Run on an H100:
 
     python tests/gpu_vae_parity_report.py            # latent 16 (B=2) and latent 64 (B=1)
 

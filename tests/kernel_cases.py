@@ -45,9 +45,9 @@ def case_tuned(tune, fn, *args):
     return err, tol, " ".join(f"{k}={v}" for k, v in tune) + ": " + desc
 
 
-PAIR = (("pair_min_tiles", 1),)     # persistent CTA-pair GEMM (gemm_pair_kernel) whatever the grid size
-NOPAIR = (("pair_min_tiles", 1 << 30),)  # single-CTA tiles on a large grid
-ATT2Q = (("attn40_2q_min_ctas", 0),)     # d=40 attention on the two-Q-tile kernel at two CTAs per SM
+PAIR = (("pair_min_tiles", 1),)     # the large-grid tiles (128 x 256 / deep rings, one CTA per SM) whatever the grid size
+NOPAIR = (("pair_min_tiles", 1 << 30),)  # the small-grid tiles (two CTAs per SM up to 128 wide) on a large grid
+ATT2Q = (("attn40_2q_min_ctas", 0),)     # d=40 attention on the register-capped variant at two CTAs per SM
 
 
 def case_gemm_ln(m, n, k, offset=0.5, seed=0):
@@ -375,28 +375,28 @@ ALL_CASES = [
     (case_conv, (2, 16, 16, 1280, 1280, True, True, 0)),   # automatic: long K -> 160-wide tiles, 4 splits
     (case_conv, (2, 8, 8, 2560, 1280, True, True, 0)),     # automatic: 8 splits
     (case_conv, (1, 16, 16, 1280, 1280, True, False, 0)),  # ControlNet at one frame: M = 256
-    # ---- persistent CTA-pair GEMM forced onto small and odd problems ----
-    (case_tuned, (PAIR, case_gemm, 512, 256, 128)),                       # 256-wide tile, 2 pairs, one K pass of 2 chunks
-    (case_tuned, (PAIR, case_gemm, 384, 320, 320, True, True)),           # odd M tiles: last pair half empty; bias+residual
-    (case_tuned, (PAIR, case_gemm, 1000, 640, 1280, True, False)),        # ragged M (TMA store clips rows)
-    (case_tuned, (PAIR, case_gemm, 300, 384, 192, True, True)),           # 128-wide tiles
-    (case_tuned, (PAIR, case_gemm, 4096, 320, 2880, True, True)),         # long K: ring wraps; 320-wide tile = full N
-    (case_tuned, (PAIR, case_gemm, 65536, 320, 320, True, True)),         # 512 tiles over 74 pairs: 7 rounds, both buffers
-    (case_tuned, (PAIR, case_gemm, 4096, 1280, 640, True, True)),         # 256-wide tiles, 5 N tiles (K too short for 320)
-    (case_tuned, (PAIR, case_gemm, 4096, 1280, 1280, True, True)),        # 320-wide tiles (2 x 160 MMAs, one accumulator)
-    (case_tuned, (PAIR, case_gemm, 1000, 640, 2560, True, True)),         # 320-wide, ragged M, 2 N tiles
-    (case_tuned, (PAIR, case_gemm, 520, 200, 128, True, True)),           # N = 200: last chunk 8 columns wide, 2nd half empty
+    # ---- the large-grid GEMM tiles forced onto small and odd problems ----
+    (case_tuned, (PAIR, case_gemm, 512, 256, 128)),                       # K of 2 chunks: too little work even when forced
+    (case_tuned, (PAIR, case_gemm, 384, 320, 320, True, True)),           # odd M tiles, 160-wide deep ring; bias+residual
+    (case_tuned, (PAIR, case_gemm, 1000, 640, 1280, True, False)),        # ragged M: rows >= M of the last tile not stored
+    (case_tuned, (PAIR, case_gemm, 300, 384, 192, True, True)),           # 128-wide deep-ring tiles
+    (case_tuned, (PAIR, case_gemm, 4096, 320, 2880, True, True)),         # long K: the 6-stage ring wraps many times
+    (case_tuned, (PAIR, case_gemm, 65536, 320, 320, True, True)),         # 512 M tiles x 2 N tiles, 160-wide
+    (case_tuned, (PAIR, case_gemm, 4096, 1280, 640, True, True)),         # 256-wide tiles, 5 N tiles
+    (case_tuned, (PAIR, case_gemm, 4096, 1280, 1280, True, True)),        # 256-wide tiles, K = 1280
+    (case_tuned, (PAIR, case_gemm, 1000, 640, 2560, True, True)),         # 160-wide, ragged M, long K
+    (case_tuned, (PAIR, case_gemm, 520, 200, 128, True, True)),           # N = 200: 128-wide tiles, the last chunk 8 columns wide
     (case_tuned, (PAIR, case_gemm_batch_bias, 2, 1024, 640, 320)),
     (case_tuned, (PAIR, case_gemm_dual, 1024, 640, 640, 320)),
     (case_tuned, (PAIR, case_gemm_strided_out, 320, 80, 768)),            # output row pitch > N
     (case_tuned, (PAIR, case_geglu, 512, 320)),
     (case_tuned, (PAIR, case_geglu, 4096, 320)),
     (case_tuned, (PAIR, case_conv, 1, 64, 64, 320, 320)),
-    (case_tuned, (PAIR, case_conv, 8, 64, 64, 320, 320, True, True)),     # full-width conv tile: 128 pairs over 74 clusters
+    (case_tuned, (PAIR, case_conv, 8, 64, 64, 320, 320, True, True)),     # eight frames at 64x64: 256 M tiles, 160-wide
     (case_tuned, (PAIR, case_conv, 2, 32, 32, 640, 640, True, True)),
-    (case_tuned, (PAIR, case_conv, 3, 8, 8, 1280, 1280, True, True)),     # 192 rows: second CTA of the pair half out of range
+    (case_tuned, (PAIR, case_conv, 3, 8, 8, 1280, 1280, True, True)),     # 192 rows: the second M tile half out of range
     (case_tuned, (PAIR, case_conv, 16, 16, 16, 1280, 1280)),
-    # ---- the same large shapes on the single-CTA tiles (what the heuristics would not pick) ----
+    # ---- the same large shapes on the small-grid tiles (what the heuristics would not pick) ----
     (case_tuned, (NOPAIR, case_gemm, 65536, 320, 320, True, True)),
     (case_tuned, (NOPAIR, case_conv, 8, 64, 64, 320, 320, True, True)),
     (case_conv_direct, (1, 64, 64, 4, 320, 1, False, True)),
@@ -408,7 +408,7 @@ ALL_CASES = [
     (case_conv_s2, (2, 32, 32, 640, 640)),
     (case_conv_s2, (2, 16, 16, 1280, 1280)),       # 8x8 output: two images per 128-row tile
     (case_conv_s2, (1, 16, 16, 1280, 1280)),       # ControlNet at one frame: half a tile
-    (case_tuned, (PAIR, case_conv_s2, 16, 64, 64, 320, 320)),   # eight frames: the pair kernel
+    (case_tuned, (PAIR, case_conv_s2, 16, 64, 64, 320, 320)),   # eight frames: the large-grid tiles
     (case_down, (2, 32, 32, 640)),
     (case_down, (1, 24, 16, 640)),
     (case_conv_im2col, (1, 12, 8, 1280, 1280)),
@@ -425,17 +425,18 @@ ALL_CASES = [
     (case_attention, (2, 8, 160, 64, 64, 64, 2)),
     (case_attention, (1, 8, 160, 16, 16, 16, 1)),
     (case_attention, (2, 8, 160, 256, 77, 0, 1, None, True)),
-    # ---- d=40 on the two-Q-tile kernel at two CTAs per SM (what large grids get) ----
+    # ---- d=40 on the register-capped variant at two CTAs per SM (what large grids get) ----
     (case_tuned, (ATT2Q, case_attention, 1, 8, 40, 4096, 4096)),
     (case_tuned, (ATT2Q, case_attention, 2, 8, 40, 1024, 1024, 1024, 2)),
     (case_tuned, (ATT2Q, case_attention, 2, 8, 40, 1024, 1024, 1024, 1, 1)),
     (case_tuned, (ATT2Q, case_attention, 2, 8, 40, 1024, 77, 0, 1, None, True)),
     (case_tuned, (ATT2Q, case_attention, 1, 8, 40, 384, 384, 128, 1)),
-    (case_attention, (16, 8, 40, 2048, 2048, 2048, 1, 8)),   # 2048 CTAs: the heuristics pick the two-Q-tile kernel
-    # ---- d=80 on the two-Q-tile kernel (one CTA, eight softmax warps per SM) ----
+    (case_attention, (16, 8, 40, 2048, 2048, 2048, 1, 8)),   # 2048 CTAs: the heuristics pick the two-CTA-per-SM variant (>= 512)
+    # ---- d=80 with the d=40 key set: d=80 has one variant (one CTA per SM), so these are ragged / odd Q-tile shapes
+    # that also check the key leaves d=80 alone ----
     (case_tuned, (ATT2Q, case_attention, 2, 8, 80, 256, 256, 256, 1)),
     (case_tuned, (ATT2Q, case_attention, 2, 8, 80, 200, 200, 0, 1)),          # ragged: the second Q tile is partly empty
     (case_tuned, (ATT2Q, case_attention, 2, 8, 80, 1024, 77, 0, 1, None, True)),
     (case_tuned, (ATT2Q, case_attention, 1, 8, 80, 384, 384, 128, 1)),        # odd number of Q tiles
-    (case_attention, (16, 8, 80, 1024, 1024, 1024, 1, 8)),   # 1024 CTAs: picked by the heuristics
+    (case_attention, (16, 8, 80, 1024, 1024, 1024, 1, 8)),   # 1024 CTAs: the eight-frame d=80 grid
 ]

@@ -23,13 +23,15 @@ def test_library_builds_loads_and_exports_every_declared_symbol():
     assert lib.mdb_abi_version() == 2 and lib.mdb_launch_count() == 0
 
 
-def test_sass_contains_blackwell_tensor_and_tma_instructions():
+def test_sass_contains_hopper_tensor_and_tma_instructions():
     from magicdance_b200 import build
     path = build.build()
     sass = subprocess.run(["cuobjdump", "-sass", path], capture_output=True, text=True, check=True).stdout
-    for mnem in ("UTCHMMA", "LDTM", "STTM", "UTMALDG", "UTCHMMA.2CTA", "UTCBAR.2CTA.MULTICAST", "UTMASTG.2D"):
-        assert mnem in sass, f"{mnem} (tcgen05 / TMA) missing from the compiled kernels"
-    assert "HMMA." not in sass.replace("UTCHMMA", ""), "legacy mma.sync path must not be present"
+    assert "arch = sm_90a" in sass
+    for mnem in ("HGMMA.64x256x16.F32", "HGMMA.64x160x16.F32", "HGMMA.64x64x16.F32", "HGMMA.64x48x16.F32",
+                 "UTMALDG.2D", "UTMALDG.3D", "UTMALDG.4D", "SYNCS.ARRIVE.TRANS64"):
+        assert mnem in sass, f"{mnem} (wgmma / TMA / mbarrier) missing from the compiled kernels"
+    assert "HMMA." not in sass.replace("HGMMA", ""), "legacy mma.sync path must not be present"
 
 
 def test_no_cuda_means_loud_failure():

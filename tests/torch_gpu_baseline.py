@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Secondary GPU baseline (BASELINE.md section 3, informative): the reference's path as plain eager PyTorch on
-one B200 — the oracle restatement (oracle/restatement.py, the same functions the CPU baseline times) moved to
+one H100 — the oracle restatement (oracle/restatement.py, the same functions the CPU baseline times) moved to
 the GPU and run under fp16 autocast with cuDNN / cuBLAS, `F.scaled_dot_product_attention` standing in for the
 xformers call the reference makes on a GPU (attention.py:242).  This is "the reference on this box": the number
 the hand-written kernels have to beat, reported next to bench.py's line, never mixed into it.
