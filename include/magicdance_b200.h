@@ -41,7 +41,8 @@ const char* mdb_last_error(void);
 int mdb_device_check(void);
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 int64_t mdb_launch_count(void);
-/* sizeof(mdb_gemm_desc) (which = 0) / sizeof(mdb_attn_desc) (which = 1): a binding checks its struct mirrors */
+/* sizeof(mdb_gemm_desc) (which = 0) / sizeof(mdb_attn_desc) (which = 1) / sizeof(mdb_attn_bwd_desc) (which = 2):
+ * a binding checks its struct mirrors */
 int64_t mdb_abi_struct_bytes(int32_t which);
 
 /* Launch heuristics, process-wide (defaults in parentheses); tests use the setter to force a kernel variant onto small
@@ -122,6 +123,43 @@ typedef struct mdb_attn_desc {
 } mdb_attn_desc;
 
 int mdb_attention_f16(const mdb_attn_desc* desc, mdb_stream_t stream);
+
+/* The same forward, which also stores the softmax statistics the backward needs:
+ *   lse : fp32 [batch][heads][nq], lse = log(sum_j exp(scale * q k_j^T)) over the row's keys of both sources
+ *         (natural log of the SCALED scores).
+ * `out` is bit-equal to mdb_attention_f16's for the same descriptor. */
+int mdb_attention_lse_f16(const mdb_attn_desc* desc, float* lse, mdb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Backward of mdb_attention_f16: the gradients of  out = softmax([Q K0^T | Q K1^T] * scale) [V0 ; V1]
+ * with respect to q, k0, v0, k1, v1 — the differentiation of CrossAttention._forward (attention.py:168-199) and of
+ * the torch.cat([x_norm1] + bank) of BasicTransformerBlock 'read' mode (attention.py:303-307), which carries the
+ * gradient of a frozen UNet into the appearance bank.  FlashAttention-2 recompute from the stored log-sum-exp.
+ * Deterministic: no atomics, two runs give bit-equal gradients.
+ *   fwd          : the forward's descriptor; fwd.out is the forward's output O
+ *   dout         : fp16 [B*Nq][heads*d], the gradient of out (row stride lddout, a multiple of 8)
+ *   lse          : from mdb_attention_lse_f16
+ *   dq           : fp16, laid out like q  [B*Nq][heads*d]          (row stride lddq)
+ *   dk0 / dk1    : fp16, laid out like k* [B*N][heads*d]           (row stride lddk*)
+ *   dvt0 / dvt1  : fp16, laid out like vt* [heads*d][B*ldv_batch]  (row stride lddvt*, the forward's ldv*_batch):
+ *                  only valid key columns are written; padding columns, and the bank rows / columns of batch
+ *                  elements b >= bank_batches, are left as they are
+ *   ws           : fp32 workspace of mdb_attention_bwd_ws_floats(batch, heads, nq) floats (no initial value needed)
+ * Shared sources (kv*_batches == 1 with batch > 1) are rejected: their gradient needs a reduction across batch
+ * elements.  Training has one bank and one prompt per sample.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct mdb_attn_bwd_desc {
+  mdb_attn_desc fwd;
+  const void* dout; int64_t lddout;
+  const float* lse;
+  void* dq; int64_t lddq;
+  void* dk0; int64_t lddk0; void* dvt0; int64_t lddvt0;
+  void* dk1; int64_t lddk1; void* dvt1; int64_t lddvt1;
+  float* ws;
+} mdb_attn_bwd_desc;
+
+int mdb_attention_bwd_f16(const mdb_attn_bwd_desc* desc, mdb_stream_t stream);
+int64_t mdb_attention_bwd_ws_floats(int32_t batch, int32_t heads, int32_t nq);
 
 /* ------------------------------------------------------------------------------------------------
  * GroupNorm(32 groups, affine) [+ SiLU], fp32 statistics, over channels-last fp16; optionally the

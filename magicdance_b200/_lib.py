@@ -38,6 +38,18 @@ class AttnDesc(C.Structure):
     ]
 
 
+class AttnBwdDesc(C.Structure):
+    _fields_ = [
+        ("fwd", AttnDesc),
+        ("dout", c_void_p), ("lddout", c_int64),
+        ("lse", c_void_p),
+        ("dq", c_void_p), ("lddq", c_int64),
+        ("dk0", c_void_p), ("lddk0", c_int64), ("dvt0", c_void_p), ("lddvt0", c_int64),
+        ("dk1", c_void_p), ("lddk1", c_int64), ("dvt1", c_void_p), ("lddvt1", c_int64),
+        ("ws", c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/magicdance_b200.h declares
 SIGNATURES = {
     "mdb_abi_version": (c_int32, []),
@@ -49,6 +61,9 @@ SIGNATURES = {
     "mdb_get_tuning": (c_int32, [c_int32]),
     "mdb_gemm_f16": (c_int32, [C.POINTER(GemmDesc), c_void_p]),
     "mdb_attention_f16": (c_int32, [C.POINTER(AttnDesc), c_void_p]),
+    "mdb_attention_lse_f16": (c_int32, [C.POINTER(AttnDesc), c_void_p, c_void_p]),
+    "mdb_attention_bwd_f16": (c_int32, [C.POINTER(AttnBwdDesc), c_void_p]),
+    "mdb_attention_bwd_ws_floats": (c_int64, [c_int32, c_int32, c_int32]),
     "mdb_groupnorm_f16": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_int32, c_int32, c_float, c_int32, c_int32, c_void_p]),
     "mdb_groupnorm_ws_floats": (c_int64, [c_int32, c_int32, c_int32]),
@@ -101,7 +116,7 @@ def load():
     if lib.mdb_abi_version() != ABI_VERSION:
         raise RuntimeError(f"magicdance_b200: ABI version mismatch ({lib.mdb_abi_version()} != {ABI_VERSION}); "
                            "rebuild the library")
-    for which, mirror in ((0, GemmDesc), (1, AttnDesc)):
+    for which, mirror in ((0, GemmDesc), (1, AttnDesc), (2, AttnBwdDesc)):
         if lib.mdb_abi_struct_bytes(which) != C.sizeof(mirror):
             raise RuntimeError(f"magicdance_b200: {mirror.__name__} mirrors {C.sizeof(mirror)} bytes, the library's "
                                f"struct has {lib.mdb_abi_struct_bytes(which)}: the binding and the library disagree")

@@ -18,6 +18,8 @@
 //              16) accumulates in registers.  O / l -> fp16 at the end.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace mdb {
@@ -55,10 +57,16 @@ struct AttnKParams {
   int bank_batches;
   float scale_log2;
 };
+// the forward that also stores the softmax statistics for the backward (attention_bwd.cu)
+struct AttnLseKParams : AttnKParams {
+  float* lse;  // fp32 [batch][heads][nq]: natural-log log-sum-exp of the row's scaled scores
+};
 
-// MINB = 2 caps the registers so that two CTAs (four MMA warpgroups) share an SM.
-template <int D, int BKV, int STAGES, int MINB>
-__global__ void __launch_bounds__(kAttnThreads, MINB) attn_wg_kernel(const __grid_constant__ AttnKParams p) {
+// MINB = 2 caps the registers so that two CTAs (four MMA warpgroups) share an SM.  LSE: also store the row
+// log-sum-exp (then the parameters are an AttnLseKParams); without it the kernel is exactly the inference one.
+template <int D, int BKV, int STAGES, int MINB, bool LSE = false>
+__global__ void __launch_bounds__(kAttnThreads, MINB)
+    attn_wg_kernel(const __grid_constant__ std::conditional_t<LSE, AttnLseKParams, AttnKParams> p) {
   using C = AttnCfg<D, BKV, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t q_bar;
@@ -194,15 +202,28 @@ __global__ void __launch_bounds__(kAttnThreads, MINB) attn_wg_kernel(const __gri
       mbar_arrive(&kv_empty[s]);  // this thread's reads of stage s (through its warpgroup's MMAs) are done
     }
 
-    float inv_l[2];
+    float inv_l[2], l_row[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float l = l_run[h];
       l += __shfl_xor_sync(0xffffffffu, l, 1);
       l += __shfl_xor_sync(0xffffffffu, l, 2);
       inv_l[h] = 1.0f / l;
+      l_row[h] = l;
     }
     const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    if constexpr (LSE) {
+      // log-sum-exp of the scaled scores: m and l are in the log2 domain, the stored value in the natural one
+      if ((lane & 3) == 0) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int q = q0 + r + 8 * h;
+          if (q < p.nq)
+            p.lse[(static_cast<long long>(b) * gridDim.y + head) * p.nq + q] =
+                (m_run[h] + log2f(l_row[h])) * 0.6931471805599453f;
+        }
+      }
+    }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int q = q0 + r + 8 * h;
@@ -228,12 +249,12 @@ static int g_attn40_2q_min_ctas = 512;
 int get_attn_tuning() { return g_attn40_2q_min_ctas; }
 void set_attn_tuning(int v) { g_attn40_2q_min_ctas = v; }
 
-template <int D, int BKV, int STAGES, int MINB>
-static int launch_attn(const AttnKParams& kp, dim3 grid, cudaStream_t st) {
+template <int D, int BKV, int STAGES, int MINB, bool LSE = false, typename P>
+static int launch_attn(const P& kp, dim3 grid, cudaStream_t st) {
   using C = AttnCfg<D, BKV, STAGES>;
   static_assert(MINB == 1 || C::kSmem <= 113 * 1024, "two CTAs per SM must fit");
   static bool attr_set = false;
-  auto kern = attn_wg_kernel<D, BKV, STAGES, MINB>;
+  auto kern = attn_wg_kernel<D, BKV, STAGES, MINB, LSE>;
   if (!attr_set) {
     MDB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem));
     attr_set = true;
@@ -243,8 +264,9 @@ static int launch_attn(const AttnKParams& kp, dim3 grid, cudaStream_t st) {
   return MDB_OK;
 }
 
+// lse != nullptr: the LSE-storing variants, with the same variant choice (and so the same `out`) as without
 template <int D, int BKV>
-static int build_and_launch(const mdb_attn_desc* a, cudaStream_t st) {
+static int build_and_launch(const mdb_attn_desc* a, float* lse, cudaStream_t st) {
   constexpr int kDV = AttnCfg<D, BKV, 1>::kDV;
   AttnKParams kp;
   memset(&kp, 0, sizeof(kp));
@@ -287,6 +309,17 @@ static int build_and_launch(const mdb_attn_desc* a, cudaStream_t st) {
   kp.bank_batches = a->n1 > 0 ? a->bank_batches : 0;
   kp.scale_log2 = a->scale * 1.4426950408889634f;
   dim3 grid((a->nq + kBQ - 1) / kBQ, a->heads, a->batch);
+  if (lse != nullptr) {
+    AttnLseKParams lp;
+    memset(&lp, 0, sizeof(lp));
+    static_cast<AttnKParams&>(lp) = kp;
+    lp.lse = lse;
+    if constexpr (D == 40) {
+      const long long ctas = (long long)grid.x * grid.y * grid.z;
+      if (ctas >= (long long)g_attn40_2q_min_ctas) return launch_attn<D, BKV, 3, 2, true>(lp, grid, st);
+    }
+    return launch_attn<D, BKV, (D == 160 ? 2 : 4), 1, true>(lp, grid, st);
+  }
   if constexpr (D == 40) {
     const long long ctas = (long long)grid.x * grid.y * grid.z;
     if (ctas >= (long long)g_attn40_2q_min_ctas) return launch_attn<D, BKV, 3, 2>(kp, grid, st);
@@ -294,11 +327,22 @@ static int build_and_launch(const mdb_attn_desc* a, cudaStream_t st) {
   return launch_attn<D, BKV, (D == 160 ? 2 : 4), 1>(kp, grid, st);
 }
 
-}  // namespace mdb
+static int attention_entry(const mdb_attn_desc* a, float* lse, cudaStream_t st) {
+  switch (a->d) {
+    case 40:
+      return build_and_launch<40, 64>(a, lse, st);
+    case 80:
+      return build_and_launch<80, 64>(a, lse, st);
+    case 160:
+      return build_and_launch<160, 64>(a, lse, st);
+    default:
+      set_error("mdb_attention_f16: head dim %d not supported (40, 80, 160)", a->d);
+      return MDB_ERR_UNSUPPORTED;
+  }
+}
 
-using namespace mdb;
-
-extern "C" int mdb_attention_f16(const mdb_attn_desc* a, mdb_stream_t stream) {
+// the forward's operand checks, shared by mdb_attention_f16, mdb_attention_lse_f16 and mdb_attention_bwd_f16
+int attention_check_desc(const mdb_attn_desc* a) {
   MDB_REQUIRE(a != nullptr, "mdb_attention_f16: null descriptor");
   MDB_REQUIRE(a->q && a->k0 && a->vt0 && a->out, "mdb_attention_f16: null operand");
   MDB_REQUIRE(a->batch > 0 && a->heads > 0 && a->nq > 0 && a->n0 > 0 && a->n1 >= 0,
@@ -309,16 +353,22 @@ extern "C" int mdb_attention_f16(const mdb_attn_desc* a, mdb_stream_t stream) {
               "mdb_attention_f16: kv1_batches must be 1 or cover bank_batches");
   MDB_REQUIRE(a->ldv0_batch >= a->n0 && a->ldv0_batch % 8 == 0, "mdb_attention_f16: ldv0_batch must be >= n0 and %% 8");
   MDB_REQUIRE(a->ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(a->out) & 15) == 0, "mdb_attention_f16: out alignment");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  switch (a->d) {
-    case 40:
-      return build_and_launch<40, 64>(a, st);
-    case 80:
-      return build_and_launch<80, 64>(a, st);
-    case 160:
-      return build_and_launch<160, 64>(a, st);
-    default:
-      set_error("mdb_attention_f16: head dim %d not supported (40, 80, 160)", a->d);
-      return MDB_ERR_UNSUPPORTED;
-  }
+  return MDB_OK;
+}
+
+}  // namespace mdb
+
+using namespace mdb;
+
+extern "C" int mdb_attention_f16(const mdb_attn_desc* a, mdb_stream_t stream) {
+  const int rc = attention_check_desc(a);
+  if (rc) return rc;
+  return attention_entry(a, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int mdb_attention_lse_f16(const mdb_attn_desc* a, float* lse, mdb_stream_t stream) {
+  const int rc = attention_check_desc(a);
+  if (rc) return rc;
+  MDB_REQUIRE(lse != nullptr, "mdb_attention_lse_f16: null lse");
+  return attention_entry(a, lse, static_cast<cudaStream_t>(stream));
 }

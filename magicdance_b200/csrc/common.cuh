@@ -209,6 +209,17 @@ __device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
   d |= static_cast<uint64_t>(1) << 62;                      // SWIZZLE_128B   [62,64)
   return d;
 }
+// MN-major operand tile (wgmma trans = 1) stored as [K rows][64 M-or-N halves] per 64-wide chunk, the same 128-byte
+// swizzled rows TMA writes: one swizzle atom is 64 M/N elements x 8 K rows (1024 B).  SBO = 1024 B steps 8 K rows,
+// LBO = `chunk_bytes` steps to the next 64 M/N elements.  A K step of 16 rows is +2048 B on the start address.
+__device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(uint32_t smem_addr, uint32_t chunk_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);   // start address  [0,14)
+  d |= static_cast<uint64_t>((chunk_bytes >> 4) & 0x3FFF) << 16;  // LBO      [16,30)
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;              // SBO = 1024 B   [32,46)
+  d |= static_cast<uint64_t>(1) << 62;                      // SWIZZLE_128B   [62,64)
+  return d;
+}
 // before the first wgmma of a batch: orders earlier register / shared-memory accesses of the warpgroup
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

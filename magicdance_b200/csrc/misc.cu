@@ -476,7 +476,16 @@ void set_attn_tuning(int v);
 extern "C" int mdb_abi_version(void) { return MDB_ABI_VERSION; }
 
 extern "C" int64_t mdb_abi_struct_bytes(int32_t which) {
-  return which == 0 ? (int64_t)sizeof(mdb_gemm_desc) : (which == 1 ? (int64_t)sizeof(mdb_attn_desc) : -1);
+  switch (which) {
+    case 0:
+      return (int64_t)sizeof(mdb_gemm_desc);
+    case 1:
+      return (int64_t)sizeof(mdb_attn_desc);
+    case 2:
+      return (int64_t)sizeof(mdb_attn_bwd_desc);
+    default:
+      return -1;
+  }
 }
 
 extern "C" int mdb_set_tuning(int32_t key, int32_t value) {

@@ -190,16 +190,11 @@ def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, re
     return out
 
 
-def attention(q, k0, vt0, n0, *, heads, d, batch, nq, out=None, kv0_batches=None, ldv0_batch=None,
-              k1=None, vt1=None, n1=0, kv1_batches=1, ldv1_batch=None, bank_batches=0, scale=None):
-    """softmax([q k0^T | q k1^T] * scale) [v0 ; v1]; k*: [rows, heads*d] (row stride free), vt*: [heads*d, cols]."""
-    lib = _lib.load()
-    for t, nm in ((q, "q"), (k0, "k0"), (vt0, "vt0")):
+def _attn_desc(q, k0, vt0, n0, *, heads, d, batch, nq, out, kv0_batches, ldv0_batch, k1, vt1, n1, kv1_batches,
+               ldv1_batch, bank_batches, scale):
+    for t, nm in ((q, "q"), (k0, "k0"), (vt0, "vt0"), (out, "out")):
         _chk(t, torch.float16, nm)
     a = _lib.AttnDesc()
-    hd = heads * d
-    if out is None:
-        out = torch.empty((batch * nq, hd), dtype=torch.float16, device=q.device)
     a.q, a.ldq = q.data_ptr(), q.stride(0)
     a.k0, a.ldk0, a.vt0, a.ldvt0 = k0.data_ptr(), k0.stride(0), vt0.data_ptr(), vt0.stride(0)
     a.n0 = n0
@@ -215,8 +210,92 @@ def attention(q, k0, vt0, n0, *, heads, d, batch, nq, out=None, kv0_batches=None
     a.out, a.ldo = out.data_ptr(), out.stride(0)
     a.batch, a.heads, a.d, a.nq = batch, heads, d, nq
     a.scale = float(d) ** -0.5 if scale is None else scale
-    _lib.check(lib.mdb_attention_f16(C.byref(a), _stream()), "attention_f16")
+    return a
+
+
+def attention(q, k0, vt0, n0, *, heads, d, batch, nq, out=None, kv0_batches=None, ldv0_batch=None,
+              k1=None, vt1=None, n1=0, kv1_batches=1, ldv1_batch=None, bank_batches=0, scale=None, lse=None):
+    """softmax([q k0^T | q k1^T] * scale) [v0 ; v1]; k*: [rows, heads*d] (row stride free), vt*: [heads*d, cols].
+    lse: optional fp32 [batch, heads, nq] that receives the row log-sum-exp of the scaled scores (natural log), for
+    attention_backward; `out` is bit-equal with and without it."""
+    lib = _lib.load()
+    _chk(q, torch.float16, "q")
+    if out is None:
+        out = torch.empty((batch * nq, heads * d), dtype=torch.float16, device=q.device)
+    a = _attn_desc(q, k0, vt0, n0, heads=heads, d=d, batch=batch, nq=nq, out=out, kv0_batches=kv0_batches,
+                   ldv0_batch=ldv0_batch, k1=k1, vt1=vt1, n1=n1, kv1_batches=kv1_batches, ldv1_batch=ldv1_batch,
+                   bank_batches=bank_batches, scale=scale)
+    if lse is None:
+        _lib.check(lib.mdb_attention_f16(C.byref(a), _stream()), "attention_f16")
+    else:
+        _chk(lse, torch.float32, "lse")
+        assert lse.is_contiguous() and lse.numel() == batch * heads * nq
+        _lib.check(lib.mdb_attention_lse_f16(C.byref(a), lse.data_ptr(), _stream()), "attention_lse_f16")
     return out
+
+
+def attention_backward(q, k0, vt0, n0, out, dout, lse, *, heads, d, batch, nq, kv0_batches=None, ldv0_batch=None,
+                       k1=None, vt1=None, n1=0, kv1_batches=1, ldv1_batch=None, bank_batches=0, scale=None):
+    """Gradients of attention() with respect to q, k0, vt0, k1, vt1 from dout (the gradient of `out`), given the
+    forward's `out` and `lse`.  Returns (dq, dk0, dvt0, dk1, dvt1) shaped like q, k0, vt0, k1, vt1 (dk1 / dvt1 are
+    None without a bank); padding columns of dvt*, and the bank rows of batch elements >= bank_batches, are zero.
+    Deterministic (csrc/attention_bwd.cu).  Shared sources (kv*_batches == 1 with batch > 1) are not supported."""
+    lib = _lib.load()
+    for t, nm in ((q, "q"), (dout, "dout")):
+        _chk(t, torch.float16, nm)
+    _chk(lse, torch.float32, "lse")
+    assert lse.is_contiguous() and lse.numel() == batch * heads * nq
+    assert dout.dim() == 2 and dout.stride(1) == 1
+    a = _lib.AttnBwdDesc()
+    a.fwd = _attn_desc(q, k0, vt0, n0, heads=heads, d=d, batch=batch, nq=nq, out=out, kv0_batches=kv0_batches,
+                       ldv0_batch=ldv0_batch, k1=k1, vt1=vt1, n1=n1, kv1_batches=kv1_batches, ldv1_batch=ldv1_batch,
+                       bank_batches=bank_batches, scale=scale)
+    dev = q.device
+    dq = torch.empty(q.shape, dtype=torch.float16, device=dev)
+    dk0 = torch.empty(k0.shape, dtype=torch.float16, device=dev)
+    dvt0 = torch.zeros(vt0.shape, dtype=torch.float16, device=dev)
+    a.dout, a.lddout, a.lse = dout.data_ptr(), dout.stride(0), lse.data_ptr()
+    a.dq, a.lddq = dq.data_ptr(), dq.stride(0)
+    a.dk0, a.lddk0, a.dvt0, a.lddvt0 = dk0.data_ptr(), dk0.stride(0), dvt0.data_ptr(), dvt0.stride(0)
+    dk1 = dvt1 = None
+    if n1 > 0:
+        dk1 = torch.zeros(k1.shape, dtype=torch.float16, device=dev)
+        dvt1 = torch.zeros(vt1.shape, dtype=torch.float16, device=dev)
+        a.dk1, a.lddk1, a.dvt1, a.lddvt1 = dk1.data_ptr(), dk1.stride(0), dvt1.data_ptr(), dvt1.stride(0)
+    ws = _workspace("attn_bwd", int(lib.mdb_attention_bwd_ws_floats(batch, heads, nq)), torch.float32, dev)
+    a.ws = ws.data_ptr()
+    _lib.check(lib.mdb_attention_bwd_f16(C.byref(a), _stream()), "attention_bwd_f16")
+    return dq, dk0, dvt0, dk1, dvt1
+
+
+class TwoSourceAttention(torch.autograd.Function):
+    """attention() as an autograd op: the forward stores the log-sum-exp, the backward runs attention_backward.
+    Positional arguments in the order of attention()'s parameters; two_source_attention() takes them as keywords."""
+
+    @staticmethod
+    def forward(ctx, q, k0, vt0, n0, heads, d, batch, nq, kv0_batches=None, ldv0_batch=None, k1=None, vt1=None, n1=0,
+                kv1_batches=1, ldv1_batch=None, bank_batches=0, scale=None):
+        kw = dict(heads=heads, d=d, batch=batch, nq=nq, kv0_batches=kv0_batches, ldv0_batch=ldv0_batch, k1=k1, vt1=vt1,
+                  n1=n1, kv1_batches=kv1_batches, ldv1_batch=ldv1_batch, bank_batches=bank_batches, scale=scale)
+        lse = torch.empty((batch, heads, nq), dtype=torch.float32, device=q.device)
+        out = attention(q, k0, vt0, n0, lse=lse, **kw)
+        ctx.save_for_backward(q, k0, vt0, k1, vt1, out, lse)
+        ctx.n0, ctx.kw = n0, {k: v for k, v in kw.items() if k not in ("k1", "vt1")}
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        q, k0, vt0, k1, vt1, out, lse = ctx.saved_tensors
+        dq, dk0, dvt0, dk1, dvt1 = attention_backward(q, k0, vt0, ctx.n0, out, dout.contiguous(), lse, k1=k1, vt1=vt1,
+                                                      **ctx.kw)
+        return (dq, dk0, dvt0) + (None,) * 7 + (dk1, dvt1) + (None,) * 5
+
+
+def two_source_attention(q, k0, vt0, n0, *, heads, d, batch, nq, kv0_batches=None, ldv0_batch=None, k1=None, vt1=None,
+                         n1=0, kv1_batches=1, ldv1_batch=None, bank_batches=0, scale=None):
+    """Differentiable attention(): gradients flow to q, k0, vt0, k1 and vt1 (TwoSourceAttention)."""
+    return TwoSourceAttention.apply(q, k0, vt0, n0, heads, d, batch, nq, kv0_batches, ldv0_batch, k1, vt1, n1,
+                                    kv1_batches, ldv1_batch, bank_batches, scale)
 
 
 GN_AUTO, GN_TWO_KERNELS, GN_CLUSTER = 0, 1, 2  # mdb_groupnorm_f16 `mode`

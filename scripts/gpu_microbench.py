@@ -63,9 +63,68 @@ def attn_case(b, d, nq, n0, n1=0):
            flops=4.0 * b * 8 * nq * (n0 + n1) * d)
 
 
+def timeit_eager(name, fn, reps=20, flops=None):
+    """CUDA events around `reps` eager calls (for torch autograd, which a CUDA graph cannot capture here)"""
+    for _ in range(3):
+        fn()
+    torch.cuda.synchronize()
+    best = 1e9
+    for _ in range(3):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        best = min(best, e0.elapsed_time(e1) * 1e3 / reps)
+    extra = f"  {flops / best / 1e6:8.1f} TFLOP/s" if flops else ""
+    print(f"{name:58s} {best:9.2f} us{extra}", flush=True)
+
+
+def attn_bwd_case(b, d, nq, n0, n1=0, heads=8):
+    """forward-with-LSE and backward (ours) against torch SDPA forward + backward on the torch.cat'ed K / V.
+    Algorithmic FLOP: forward 4 nq nk d, backward 10 nq nk d per head (nk = n0 + n1)."""
+    import torch.nn.functional as F
+    c = heads * d
+    nk = n0 + n1
+    ldv = (n0 + 7) // 8 * 8
+    q, k0, vt0, dout = h(b * nq, c), h(b * n0, c), h(c, b * ldv), h(b * nq, c)
+    kw = dict(heads=heads, d=d, batch=b, nq=nq, ldv0_batch=ldv)
+    if n1:
+        kw.update(k1=h(b * n1, c), vt1=h(c, b * n1), n1=n1, kv1_batches=b, bank_batches=b)
+    lse = torch.empty(b, heads, nq, device=D)
+    out = ops.attention(q, k0, vt0, n0, lse=lse, **kw)
+    fl_f, fl_b = 4.0 * b * heads * nq * nk * d, 10.0 * b * heads * nq * nk * d
+    tag = f"B={b} d={d} nq={nq} n0={n0} n1={n1}"
+    timeit(f"ours fwd+lse {tag}", lambda: ops.attention(q, k0, vt0, n0, out=out, lse=lse, **kw), flops=fl_f)
+    timeit(f"ours bwd     {tag}", lambda: ops.attention_backward(q, k0, vt0, n0, out, dout, lse, **kw), flops=fl_b)
+    # torch: [B, heads, tokens, d] with the two sources concatenated
+    qt = torch.randn(b, heads, nq, d, device=D, dtype=torch.float16, requires_grad=True)
+    kt = torch.randn(b, heads, nk, d, device=D, dtype=torch.float16, requires_grad=True)
+    vt = torch.randn(b, heads, nk, d, device=D, dtype=torch.float16, requires_grad=True)
+    g = torch.randn(b, heads, nq, d, device=D, dtype=torch.float16)
+    with torch.no_grad():
+        timeit_eager(f"sdpa fwd     {tag}", lambda: F.scaled_dot_product_attention(qt, kt, vt), flops=fl_f)
+    timeit_eager(f"sdpa fwd+bwd {tag}",
+                 lambda: torch.autograd.grad(F.scaled_dot_product_attention(qt, kt, vt), (qt, kt, vt), g),
+                 flops=fl_f + fl_b)
+
+
 def main():
     which = sys.argv[1] if len(sys.argv) > 1 else "all"
     ops.ensure_device()
+    if which == "attn_bwd":
+        import subprocess
+        smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True).stdout.strip()
+        print(f"GPU: {torch.cuda.get_device_name()} | nvidia-smi: {smi}", flush=True)
+        # BASELINE config 5: 4 samples at latent 64x64, 8 heads; self + bank at every level, the text source at 64x64
+        attn_bwd_case(4, 40, 4096, 4096, 4096)
+        attn_bwd_case(4, 80, 1024, 1024, 1024)
+        attn_bwd_case(4, 160, 256, 256, 256)
+        attn_bwd_case(4, 160, 64, 64, 64)
+        attn_bwd_case(4, 40, 4096, 77)
+        return
     if which in ("all", "gemm"):
         for m, n, k in ((128, 160, 64), (128, 160, 640), (128, 160, 2560), (128, 1280, 1280)):
             gemm_case(m, n, k, res=False, bias=False)
