@@ -41,8 +41,8 @@ const char* mdb_last_error(void);
 int mdb_device_check(void);
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 int64_t mdb_launch_count(void);
-/* sizeof(mdb_gemm_desc) (which = 0) / sizeof(mdb_attn_desc) (which = 1) / sizeof(mdb_attn_bwd_desc) (which = 2):
- * a binding checks its struct mirrors */
+/* sizeof(mdb_gemm_desc) (which = 0) / sizeof(mdb_attn_desc) (which = 1) / sizeof(mdb_attn_bwd_desc) (which = 2) /
+ * sizeof(mdb_gemm_bwd_desc) (which = 3): a binding checks its struct mirrors */
 int64_t mdb_abi_struct_bytes(int32_t which);
 
 /* Launch heuristics, process-wide (defaults in parentheses); tests use the setter to force a kernel variant onto small
@@ -97,6 +97,46 @@ typedef struct mdb_gemm_desc {
 } mdb_gemm_desc;
 
 int mdb_gemm_f16(const mdb_gemm_desc* desc, mdb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Backward of mdb_gemm_f16 (EPI_NONE, no ln_u): with D = A B^T (+ bias + residual) and dD its gradient,
+ *   dA    = dD B       reduces over N: the input gradient of nn.Linear / 1x1 conv (attention.py:154-161,342-361),
+ *                      and in conv mode of the 3x3 conv_nd (openaimodel.py:225,249-252,175) — col2im by gather;
+ *   dB    = dD^T A     reduces over M (tokens / pixels): the weight gradient of the same layers;
+ *   dbias = column sums of dD (per segment of rows_per_batch rows when bias_batch_stride != 0: the gradient of the
+ *           per-sample timestep bias of ResBlock.emb_layers, openaimodel.py:238-244,262-263).
+ * The residual's gradient is dD itself.  Deterministic: no atomics; split reductions go through fp32 slabs summed in
+ * a fixed order, so two calls give bit-equal results.  Nothing is transposed in memory: B (dA) and both operands
+ * (dB) are read MN-major by wgmma from the TMA tiles.
+ *   fwd     : the forward's descriptor; its a / a2 / b / geometry / bias geometry are used, d / residual / bias
+ *             pointers ignored; fwd.splits is the split count of the dA reduction (0 automatic, 1 none)
+ *   dd      : fp16 [M][N], row stride lddd (a multiple of 8, 16-byte aligned base)
+ *   da      : [M][k1] (conv: NHWC like fwd.a), da2: [M][K - k1] (the a2 columns); db: [N][K] (conv: [O][kh][kw][I])
+ *   dbias   : fp32, dbias[(row / rows_per_batch) * bias_batch_stride + col] like the forward's bias
+ *   NULL    = that gradient is not wanted; *_dtype MDB_DTYPE_F16 | MDB_DTYPE_F32; *_accumulate != 0 adds the
+ *             gradient to the destination's contents instead of overwriting them
+ *   splits  : split count of the dB reduction over M (0 automatic, 1 none)
+ *   ws      : fp32 workspace of mdb_gemm_bwd_ws_floats(desc) floats (no initial value needed)
+ * Stride-2 convs and latents whose rows do not tile into the TMA boxes (e.g. 12x8) take dA through an fp32 column
+ * buffer and a gather kernel; non-tiling latents take dB through mdb_im2col3x3_f16.
+ * ---------------------------------------------------------------------------------------------- */
+#define MDB_DTYPE_F16 0
+#define MDB_DTYPE_F32 1
+
+typedef struct mdb_gemm_bwd_desc {
+  mdb_gemm_desc fwd;
+  const void* dd; int64_t lddd;
+  void* da; int64_t ldda; int32_t da_dtype; int32_t da_accumulate;
+  void* da2; int64_t ldda2; int32_t da2_dtype; int32_t da2_accumulate;
+  void* db; int64_t lddb; int32_t db_dtype; int32_t db_accumulate;
+  float* dbias; int32_t dbias_accumulate;
+  int32_t splits;
+  float* ws;
+} mdb_gemm_bwd_desc;
+
+int mdb_gemm_bwd_f16(const mdb_gemm_bwd_desc* desc, mdb_stream_t stream);
+/* workspace floats mdb_gemm_bwd_f16 needs for this descriptor; negative MDB_ERR_* for a descriptor it rejects */
+int64_t mdb_gemm_bwd_ws_floats(const mdb_gemm_bwd_desc* desc);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused attention, FlashAttention-style tile loop on wgmma, with TWO key/value sources whose

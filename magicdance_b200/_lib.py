@@ -50,6 +50,19 @@ class AttnBwdDesc(C.Structure):
     ]
 
 
+class GemmBwdDesc(C.Structure):
+    _fields_ = [
+        ("fwd", GemmDesc),
+        ("dd", c_void_p), ("lddd", c_int64),
+        ("da", c_void_p), ("ldda", c_int64), ("da_dtype", c_int32), ("da_accumulate", c_int32),
+        ("da2", c_void_p), ("ldda2", c_int64), ("da2_dtype", c_int32), ("da2_accumulate", c_int32),
+        ("db", c_void_p), ("lddb", c_int64), ("db_dtype", c_int32), ("db_accumulate", c_int32),
+        ("dbias", c_void_p), ("dbias_accumulate", c_int32),
+        ("splits", c_int32),
+        ("ws", c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/magicdance_b200.h declares
 SIGNATURES = {
     "mdb_abi_version": (c_int32, []),
@@ -60,6 +73,8 @@ SIGNATURES = {
     "mdb_set_tuning": (c_int32, [c_int32, c_int32]),
     "mdb_get_tuning": (c_int32, [c_int32]),
     "mdb_gemm_f16": (c_int32, [C.POINTER(GemmDesc), c_void_p]),
+    "mdb_gemm_bwd_f16": (c_int32, [C.POINTER(GemmBwdDesc), c_void_p]),
+    "mdb_gemm_bwd_ws_floats": (c_int64, [C.POINTER(GemmBwdDesc)]),
     "mdb_attention_f16": (c_int32, [C.POINTER(AttnDesc), c_void_p]),
     "mdb_attention_lse_f16": (c_int32, [C.POINTER(AttnDesc), c_void_p, c_void_p]),
     "mdb_attention_bwd_f16": (c_int32, [C.POINTER(AttnBwdDesc), c_void_p]),
@@ -116,7 +131,7 @@ def load():
     if lib.mdb_abi_version() != ABI_VERSION:
         raise RuntimeError(f"magicdance_b200: ABI version mismatch ({lib.mdb_abi_version()} != {ABI_VERSION}); "
                            "rebuild the library")
-    for which, mirror in ((0, GemmDesc), (1, AttnDesc), (2, AttnBwdDesc)):
+    for which, mirror in ((0, GemmDesc), (1, AttnDesc), (2, AttnBwdDesc), (3, GemmBwdDesc)):
         if lib.mdb_abi_struct_bytes(which) != C.sizeof(mirror):
             raise RuntimeError(f"magicdance_b200: {mirror.__name__} mirrors {C.sizeof(mirror)} bytes, the library's "
                                f"struct has {lib.mdb_abi_struct_bytes(which)}: the binding and the library disagree")

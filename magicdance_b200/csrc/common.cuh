@@ -44,6 +44,10 @@ void set_error(const char* fmt, ...);
 // byte stride of dims[i+1].  Returns 0 on success.
 int make_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                   const uint64_t* strides_bytes, const uint32_t* box);
+// the same with a chosen swizzle and TMA element strides (nullptr = 1 along every dimension)
+int make_tmap_f16_sw(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle,
+                     const uint32_t* elem_strides = nullptr);
 
 // ----------------------------------------------------------------------------------------------
 // device-side PTX wrappers

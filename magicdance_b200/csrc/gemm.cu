@@ -511,9 +511,9 @@ __global__ void splitk_finalize_kernel(GemmKParams p) {
 // ------------------------------------------------------------------------------------------------
 static PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
 
-static int make_tmap_f16_sw(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                            const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle,
-                            const uint32_t* elem_strides = nullptr) {
+int make_tmap_f16_sw(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle,
+                     const uint32_t* elem_strides) {
   if (g_encode == nullptr) {
     void* fn = nullptr;
     cudaDriverEntryPointQueryResult qres;

@@ -483,6 +483,8 @@ extern "C" int64_t mdb_abi_struct_bytes(int32_t which) {
       return (int64_t)sizeof(mdb_attn_desc);
     case 2:
       return (int64_t)sizeof(mdb_attn_bwd_desc);
+    case 3:
+      return (int64_t)sizeof(mdb_gemm_bwd_desc);
     default:
       return -1;
   }

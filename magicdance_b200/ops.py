@@ -190,6 +190,164 @@ def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, re
     return out
 
 
+_DTYPES = {torch.float16: 0, torch.float32: 1}  # MDB_DTYPE_F16 / MDB_DTYPE_F32
+
+
+def _grad_out(t, shape, dtype, device, name):
+    """the destination of one gradient: `t` (2-D, unit column stride) or a new tensor"""
+    if t is None:
+        t = torch.empty(shape, dtype=dtype, device=device)
+    if t.dtype not in _DTYPES:
+        raise RuntimeError(f"magicdance_b200: {name} must be float16 or float32, got {t.dtype}")
+    _chk(t, t.dtype, name)
+    assert t.dim() == 2 and t.stride(1) == 1 and tuple(t.shape) == tuple(shape), (name, t.shape, shape)
+    return t
+
+
+def gemm_backward(a, w, dd, *, a2=None, conv=None, conv_stride=1, bias_batch_stride=0, rows_per_batch=0, splits=0,
+                  db_splits=0, m=None, grads=("a", "b"), da_dtype=torch.float16, db_dtype=torch.float32, out_da=None,
+                  out_da2=None, out_db=None, out_dbias=None, accumulate=(), epilogue=EPI_NONE, ln_u=None):
+    """Gradients of D = gemm(a, w, ...) from dd = dL/dD (fp16 [M, N], row stride a multiple of 8), csrc/gemm_bwd.cu:
+    dA = dd w, dW = dd^T a, dbias = column sums of dd (per batch element: [M / rows_per_batch, bias_batch_stride]).
+    a, w, a2, conv, conv_stride, bias_batch_stride, rows_per_batch and m are gemm()'s arguments; `splits` splits the
+    reduction of dA (over N), `db_splits` that of dW (over M): 0 automatic, 1 none.  `grads` names the gradients to
+    compute among "a" (dA, and dA2 with a2), "b" and "bias".  Each goes to its out_* tensor when given (its dtype is
+    then the gradient's dtype) or to a new one of da_dtype / db_dtype (dbias: fp32); names in `accumulate` ("a",
+    "a2", "b", "bias") add into the out_* tensor instead of overwriting it.  Returns (da, da2, dw, dbias), None for a
+    gradient not requested.  Deterministic; GEGLU and ln_u GEMMs are rejected."""
+    lib = _lib.load()
+    _chk(a, torch.float16, "a")
+    _chk(w, torch.float16, "w")
+    _chk(dd, torch.float16, "dd")
+    assert dd.dim() == 2 and dd.stride(1) == 1
+    dev = a.device
+    g = _lib.GemmBwdDesc()
+    f = g.fwd
+    n, k = w.shape
+    if conv is not None:
+        nb, h, wd, c = conv
+        assert conv_stride in (1, 2) and a.is_contiguous() and a.numel() == nb * h * wd * c
+        m = nb * ((h - 1) // conv_stride + 1) * ((wd - 1) // conv_stride + 1)
+        f.conv, f.nb, f.h, f.w, f.c = conv_stride, nb, h, wd, c
+        f.a, f.lda, f.k1 = a.data_ptr(), c, k
+        da_shape, k1 = (nb * h * wd, c), k
+    else:
+        assert a.dim() == 2 and a.stride(1) == 1
+        m = a.shape[0] if m is None else m
+        k1 = a.shape[1]
+        f.a, f.lda, f.k1 = a.data_ptr(), a.stride(0), k1
+        if a2 is not None:
+            _chk(a2, torch.float16, "a2")
+            assert a2.dim() == 2 and a2.stride(1) == 1 and a2.shape[0] == a.shape[0] and k1 + a2.shape[1] == k
+            f.a2, f.lda2 = a2.data_ptr(), a2.stride(0)
+        else:
+            assert k1 == k, (a.shape, w.shape)
+        da_shape = (m, k1)
+    assert w.stride(1) == 1 and dd.shape[0] >= m and dd.shape[1] == n, (dd.shape, m, n)
+    f.b, f.ldb = w.data_ptr(), w.stride(0)
+    f.m, f.n, f.k, f.epilogue, f.splits = m, n, k, epilogue, splits
+    f.bias_batch_stride, f.rows_per_batch = bias_batch_stride, rows_per_batch
+    if ln_u is not None:
+        f.ln_u = ln_u.data_ptr()
+    g.dd, g.lddd, g.splits = dd.data_ptr(), dd.stride(0), db_splits
+    acc = set(accumulate)
+    da = da2 = dw = dbias = None
+    if "a" in grads:
+        da = _grad_out(out_da, da_shape, da_dtype, dev, "out_da")
+        g.da, g.ldda, g.da_dtype, g.da_accumulate = da.data_ptr(), da.stride(0), _DTYPES[da.dtype], "a" in acc
+        if a2 is not None:
+            da2 = _grad_out(out_da2, (m, k - k1), da_dtype, dev, "out_da2")
+            g.da2, g.ldda2, g.da2_dtype = da2.data_ptr(), da2.stride(0), _DTYPES[da2.dtype]
+            g.da2_accumulate = "a2" in acc
+    if "b" in grads:
+        dw = _grad_out(out_db, (n, k), db_dtype, dev, "out_db")
+        g.db, g.lddb, g.db_dtype, g.db_accumulate = dw.data_ptr(), dw.stride(0), _DTYPES[dw.dtype], "b" in acc
+    if "bias" in grads:
+        shape = (n,) if bias_batch_stride == 0 else (-(-m // rows_per_batch), bias_batch_stride)
+        dbias = torch.empty(shape, dtype=torch.float32, device=dev) if out_dbias is None else out_dbias
+        _chk(dbias, torch.float32, "out_dbias")
+        assert dbias.is_contiguous() and tuple(dbias.shape) == shape, (dbias.shape, shape)
+        g.dbias, g.dbias_accumulate = dbias.data_ptr(), "bias" in acc
+    need = int(lib.mdb_gemm_bwd_ws_floats(C.byref(g)))
+    if need < 0:
+        _lib.check(need, "gemm_bwd_f16")
+    g.ws = _workspace("gemm_bwd", need, torch.float32, dev).data_ptr()
+    _lib.check(lib.mdb_gemm_bwd_f16(C.byref(g), _stream()), "gemm_bwd_f16")
+    return da, da2, dw, dbias
+
+
+def _rows8(t):
+    """t as a [rows, cols] fp16 matrix whose row stride is a multiple of 8 (the kernels' alignment), copied if not"""
+    if t.stride(1) == 1 and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0:
+        return t
+    buf = torch.zeros((t.shape[0], (t.shape[1] + 7) // 8 * 8), dtype=t.dtype, device=t.device)
+    buf[:, :t.shape[1]] = t
+    return buf[:, :t.shape[1]]
+
+
+class TcGemm(torch.autograd.Function):
+    """gemm() (EPI_NONE) as an autograd op.  Each operand is an fp16 activation (gradient fp16) or the fp16 packed
+    copy of an fp32 parameter passed with it (a_param / w_param: the gradient, fp32, goes to the parameter in its own
+    layout — Linear (out, in); Conv2d OIHW as a view of the [O][kh][kw][I] result).  The bias (fp32 row or per-batch
+    [batch, N]) gets its fp32 gradient, the residual dD.  Positional arguments in tc_gemm()'s order."""
+
+    @staticmethod
+    def forward(ctx, a, a_param, w, w_param, bias, residual, a2, bias_batch_stride, rows_per_batch, conv, conv_stride,
+                splits, m):
+        n = w.shape[0]
+        if conv is not None:
+            mm = conv[0] * ((conv[1] - 1) // conv_stride + 1) * ((conv[2] - 1) // conv_stride + 1)
+        else:
+            mm = a.shape[0] if m is None else m
+        out = torch.empty((mm, (n + 7) // 8 * 8), dtype=torch.float16, device=a.device)[:, :n]
+        gemm(a, w, out=out, bias=bias, bias_batch_stride=bias_batch_stride, rows_per_batch=rows_per_batch,
+             residual=residual, a2=a2, conv=conv, conv_stride=conv_stride, splits=splits, m=m)
+        ctx.save_for_backward(a, a_param, w, w_param, a2)
+        ctx.kw = dict(conv=conv, conv_stride=conv_stride, bias_batch_stride=bias_batch_stride,
+                      rows_per_batch=rows_per_batch, m=m)
+        ctx.bias_shape = None if bias is None else bias.shape
+        ctx.has_residual = residual is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        a, a_param, w, w_param, a2 = ctx.saved_tensors
+        dd = _rows8(dout)
+        need = ctx.needs_input_grad
+        grads = [nm for nm, want in (("a", need[0] or need[1] or need[6]), ("b", need[2] or need[3]),
+                                     ("bias", need[4])) if want]
+        da, da2, dw, dbias = gemm_backward(
+            a, w, dd, a2=a2, grads=grads, da_dtype=torch.float32 if a_param is not None else torch.float16,
+            db_dtype=torch.float32 if w_param is not None else torch.float16, **ctx.kw)
+        g_a = g_ap = g_w = g_wp = None
+        if da is not None:
+            if a_param is not None:
+                g_ap = da.view(a_param.shape)
+            else:
+                g_a = da.view(a.shape)
+        if dw is not None:
+            if w_param is not None:
+                # Conv2d OIHW: the kernel's [O][kh][kw][I] rows, viewed
+                g_wp = dw.view(w_param.shape[0], 3, 3, -1).permute(0, 3, 1, 2) if w_param.dim() == 4 else dw
+            else:
+                g_w = dw
+        g_bias = dbias.view(ctx.bias_shape) if dbias is not None else None
+        g_res = dout if ctx.has_residual else None
+        return g_a, g_ap, g_w, g_wp, g_bias, g_res, da2, None, None, None, None, None, None
+
+
+def tc_gemm(a, w, *, a_param=None, w_param=None, bias=None, bias_batch_stride=0, rows_per_batch=0, residual=None,
+            a2=None, conv=None, conv_stride=1, splits=0, m=None, epilogue=EPI_NONE, ln_u=None):
+    """Differentiable gemm() (TcGemm).  GEGLU and the folded LayerNorm have no backward kernel and are refused here,
+    before anything runs."""
+    if epilogue != EPI_NONE:
+        raise RuntimeError("magicdance_b200.tc_gemm: the GEGLU epilogue has no backward kernel")
+    if ln_u is not None:
+        raise RuntimeError("magicdance_b200.tc_gemm: the folded LayerNorm (ln_u) has no backward kernel")
+    return TcGemm.apply(a, a_param, w, w_param, bias, residual, a2, bias_batch_stride, rows_per_batch, conv,
+                        conv_stride, splits, m)
+
+
 def _attn_desc(q, k0, vt0, n0, *, heads, d, batch, nq, out, kv0_batches, ldv0_batch, k1, vt1, n1, kv1_batches,
                ldv1_batch, bank_batches, scale):
     for t, nm in ((q, "q"), (k0, "k0"), (vt0, "vt0"), (out, "out")):

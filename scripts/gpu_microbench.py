@@ -110,9 +110,62 @@ def attn_bwd_case(b, d, nq, n0, n1=0, heads=8):
                  flops=fl_f + fl_b)
 
 
+def gemm_bwd_case(m, n, k, conv=None, stride=1):
+    """our dA, dW and dbias (ops.gemm_backward, one gradient per call) against cuDNN's convolution_backward on fp16
+    channels-last (convs) or cuBLAS through torch.autograd.grad of F.linear minus its forward (Linear).
+    Algorithmic FLOP: 2 M N K for each of dA and dW."""
+    import torch.nn.functional as F
+    if conv is not None:
+        nb, hh, ww = conv
+        c = k // 9
+        m = nb * ((hh - 1) // stride + 1) * ((ww - 1) // stride + 1)
+        a, kw = h(nb * hh * ww, c), dict(conv=(nb, hh, ww, c), conv_stride=stride)
+        tag = f"conv{stride} B={nb} {hh}x{ww} {c}->{n}"
+    else:
+        a, kw = h(m, k), {}
+        tag = f"linear m={m} n={n} k={k}"
+    w, dd = h(n, k), h(m, n)
+    fl = 2.0 * m * n * k
+    da = torch.empty(a.shape, dtype=torch.float16, device=D)
+    dw = torch.empty(n, k, device=D)
+    db = torch.empty(n, device=D)
+    timeit(f"ours dA    {tag}", lambda: ops.gemm_backward(a, w, dd, grads=("a",), out_da=da, **kw), flops=fl)
+    timeit(f"ours dW    {tag}", lambda: ops.gemm_backward(a, w, dd, grads=("b",), out_db=dw, **kw), flops=fl)
+    timeit(f"ours dbias {tag}", lambda: ops.gemm_backward(a, w, dd, grads=("bias",), out_dbias=db, **kw),
+           bytes_=2.0 * m * n)
+    if conv is not None:
+        x = a.view(nb, hh, ww, c).permute(0, 3, 1, 2)  # NCHW view of NHWC memory: channels-last
+        wt = w.view(n, 3, 3, c).permute(0, 3, 1, 2)
+        g = dd.view(nb, -1, n).view(nb, (hh - 1) // stride + 1, (ww - 1) // stride + 1, n).permute(0, 3, 1, 2)
+        cb = lambda mask: torch.ops.aten.convolution_backward(g, x, wt, [n], [stride] * 2, [1, 1], [1, 1], False,
+                                                              [0, 0], 1, mask)
+        timeit_eager(f"cudnn dA   {tag}", lambda: cb([True, False, False]), flops=fl)
+        timeit_eager(f"cudnn dW   {tag}", lambda: cb([False, True, False]), flops=fl)
+    else:
+        at, wt = a.clone().requires_grad_(), w.clone().requires_grad_()
+        with torch.no_grad():
+            timeit_eager(f"cublas fwd        {tag}", lambda: F.linear(a, w), flops=fl)
+        timeit_eager(f"cublas fwd+dA+dW  {tag} (subtract fwd)",
+                     lambda: torch.autograd.grad(F.linear(at, wt), (at, wt), dd), flops=3 * fl)
+
+
 def main():
     which = sys.argv[1] if len(sys.argv) > 1 else "all"
     ops.ensure_device()
+    if which == "gemm_bwd":
+        import subprocess
+        smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True).stdout.strip()
+        print(f"GPU: {torch.cuda.get_device_name()} | nvidia-smi: {smi}", flush=True)
+        # BASELINE config 5: 4 samples at latent 64x64 (16384 tokens); the UNet's Linear and 3x3 conv shapes
+        for m, n, k in ((16384, 320, 320), (16384, 2560, 320), (16384, 320, 1280), (1024, 1280, 1280), (308, 320, 768)):
+            gemm_bwd_case(m, n, k)
+        for hw, cin, cout in ((64, 320, 320), (32, 640, 640), (16, 1280, 1280), (8, 1280, 1280), (8, 2560, 1280),
+                              (64, 960, 320)):
+            gemm_bwd_case(0, cout, 9 * cin, conv=(4, hw, hw))
+        for hw, c in ((64, 320), (32, 640), (16, 1280)):
+            gemm_bwd_case(0, c, 9 * c, conv=(4, hw, hw), stride=2)
+        return
     if which == "attn_bwd":
         import subprocess
         smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],

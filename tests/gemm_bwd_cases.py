@@ -1,0 +1,149 @@
+"""Numerics cases of the GEMM / implicit-GEMM convolution backward (ops.gemm_backward): each case runs the backward on
+the GPU and returns (error, tolerance, description) against torch fp32 autograd of F.linear / F.conv2d computed from
+the SAME fp16-rounded inputs.  Run by tests/test_gemm_bwd_gpu.py; the same (error, tolerance, description) contract
+as tests/kernel_cases.py.  The error is the largest rel-L2 over the requested gradients."""
+import torch
+import torch.nn.functional as F
+
+from magicdance_b200 import ops
+from tests.kernel_cases import DEV, _rand, rel
+
+TOL = 2e-3  # the forward GEMM's gate
+_DT = {"f16": torch.float16, "f32": torch.float32}
+
+
+def padded(rows, cols, seed, scale=1.0):
+    """fp16 [rows, cols] whose row stride is rounded up to a multiple of 8 (the kernels' alignment; N = 77)"""
+    buf = torch.zeros(rows, (cols + 7) // 8 * 8, dtype=torch.float16, device=DEV)
+    buf[:, :cols] = _rand(rows, cols, seed=seed, scale=scale).half()
+    return buf[:, :cols]
+
+
+def case_gemm_bwd(m, n, k, conv=None, stride=1, k2=0, bias=None, rows_per_batch=0, grads=("a", "b"), da_dtype="f16",
+                  db_dtype="f32", accumulate=(), splits=0, db_splits=0, seed=0):
+    """m, n, k: the forward's M x N x K (conv=(nb, h, w): k = 9c, m is derived); k2: columns of a second source a2;
+    bias: None | "row" | "batch" (per segment of rows_per_batch rows); accumulate: gradients added into random
+    destinations."""
+    if conv is not None:
+        nb, h, w_ = conv
+        c = k // 9
+        ho, wo = (h - 1) // stride + 1, (w_ - 1) // stride + 1
+        m = nb * ho * wo
+        a = _rand(nb * h * w_, c, seed=seed).half()
+        a2 = None
+    else:
+        a = _rand(m, k - k2, seed=seed).half()
+        a2 = _rand(m, k2, seed=seed + 4).half() if k2 else None
+    w = _rand(n, k, seed=seed + 1, scale=k ** -0.5).half()
+    dd = padded(m, n, seed + 2)
+    kw = dict(a2=a2, splits=splits, db_splits=db_splits, grads=tuple(grads) + (("bias",) if bias else ()),
+              da_dtype=_DT[da_dtype], db_dtype=_DT[db_dtype], accumulate=accumulate)
+    if conv is not None:
+        kw.update(conv=(nb, h, w_, c), conv_stride=stride)
+    segs = 1
+    if bias == "batch":
+        segs = -(-m // rows_per_batch)
+        kw.update(bias_batch_stride=n, rows_per_batch=rows_per_batch)
+    # destinations to accumulate into start from random contents
+    init = {}
+    da_shape = a.shape
+    if "a" in accumulate:
+        init["a"] = _rand(*da_shape, seed=seed + 5).to(_DT[da_dtype])
+        kw["out_da"] = init["a"].clone()
+    if "b" in accumulate:
+        init["b"] = _rand(n, k, seed=seed + 6).to(_DT[db_dtype])
+        kw["out_db"] = init["b"].clone()
+    if "bias" in accumulate:
+        init["bias"] = _rand(*((n,) if bias == "row" else (segs, n)), seed=seed + 7).float()
+        kw["out_dbias"] = init["bias"].clone()
+    da, da2, dw, dbias = ops.gemm_backward(a, w, dd, **kw)
+
+    with torch.enable_grad():  # other tests switch autograd off process-wide
+        wf = w.float().requires_grad_()
+        if conv is not None:
+            xf = a.float().view(nb, h, w_, c).permute(0, 3, 1, 2).contiguous().requires_grad_()
+            wc = wf.view(n, 3, 3, c).permute(0, 3, 1, 2)
+            out = F.conv2d(xf, wc, stride=stride, padding=1).permute(0, 2, 3, 1).reshape(m, n)
+            inputs = [xf]
+        else:
+            af = a.float().requires_grad_()
+            a2f = a2.float().requires_grad_() if a2 is not None else None
+            out = F.linear(torch.cat([af, a2f], 1) if a2 is not None else af, wf)
+            inputs = [af] + ([a2f] if a2 is not None else [])
+        (out * dd.float()).sum().backward()
+    ddf = dd.float()
+    refs = {}
+    if conv is not None:
+        refs["a"] = xf.grad.permute(0, 2, 3, 1).reshape(nb * h * w_, c)
+    else:
+        refs["a"] = inputs[0].grad
+        if a2 is not None:
+            refs["a2"] = inputs[1].grad
+    refs["b"] = wf.grad
+    if bias == "row":
+        refs["bias"] = ddf.sum(0)
+    elif bias == "batch":
+        refs["bias"] = torch.stack([ddf[s * rows_per_batch:(s + 1) * rows_per_batch].sum(0) for s in range(segs)])
+    got = {"a": da, "a2": da2, "b": dw, "bias": dbias}
+    errs = {}
+    for name, ref in refs.items():
+        if got[name] is None:
+            continue
+        base = init.get(name)
+        errs[name] = rel(got[name].float(), ref if base is None else base.float() + ref)
+    shape = f"conv{stride} nb={conv[0]} {conv[1]}x{conv[2]} {c}->{n}" if conv is not None else f"m={m} n={n} k={k}"
+    desc = (f"gemm backward {shape} k2={k2} bias={bias} da={da_dtype} db={db_dtype} acc={','.join(accumulate)} "
+            f"splits={splits}/{db_splits}: rel-L2 " + " ".join(f"d{nm} {e:.2e}" for nm, e in errs.items()))
+    return max(errs.values()), TOL, desc
+
+
+# keyword arguments of case_gemm_bwd; config-5 sizes are batch 4 at a 64x64 latent
+CASES = [
+    # Linear at 64x64 x batch 4 (M = 16384 tokens)
+    dict(m=16384, n=320, k=320, bias="row"),                 # attn q/k/v/out, proj_in/out
+    dict(m=16384, n=2560, k=320),                            # GEGLU proj (dD = the pre-activation gradient)
+    dict(m=16384, n=320, k=1280),                            # FF out
+    dict(m=1024, n=1280, k=1280, bias="row"),
+    # text projections to_k / to_v of the cross-attention: 4 x 77 tokens, K = 768, weight gradient only
+    dict(m=308, n=320, k=768, grads=("b",)),
+    dict(m=308, n=1280, k=768, grads=("b",)),
+    # ragged M
+    dict(m=1000, n=320, k=640, bias="row"),
+    # the V^T form gemm(W_v, x): dA is the weight gradient (fp32, reduces over tokens), dB the activation's (fp16)
+    dict(m=320, n=4096, k=320, da_dtype="f32", db_dtype="f16"),
+    dict(m=320, n=77, k=768, da_dtype="f32", db_dtype="f16"),  # text V^T: N = 77
+    # dual source: 640 + 320 channels of the skip concat -> 320
+    dict(m=4096, n=320, k=960, k2=320, bias="row"),
+    # per-batch bias (timestep embedding), 4 segments
+    dict(m=4096, n=640, k=640, bias="batch", rows_per_batch=1024),
+    # accumulate into the destination
+    dict(m=2048, n=320, k=320, accumulate=("a",)),
+    dict(m=2048, n=320, k=320, bias="row", da_dtype="f32", accumulate=("a", "b", "bias")),
+    # forced splits of both reductions: counts the automatic choice does not take, and none
+    dict(m=1024, n=1280, k=1280, splits=3, db_splits=5),
+    dict(m=1024, n=1280, k=1280, splits=1, db_splits=1),
+    dict(m=0, n=320, k=9 * 320, conv=(1, 32, 32), splits=2, db_splits=3),
+    dict(m=0, n=320, k=9 * 320, conv=(1, 32, 32), splits=1, db_splits=1),
+]
+for _nb in (1, 4):  # 3x3 stride 1 (implicit dA and dB)
+    CASES += [
+        dict(m=0, n=320, k=9 * 320, conv=(_nb, 64, 64), bias="row"),
+        dict(m=0, n=640, k=9 * 640, conv=(_nb, 32, 32)),
+        dict(m=0, n=1280, k=9 * 1280, conv=(_nb, 16, 16)),
+        dict(m=0, n=1280, k=9 * 1280, conv=(_nb, 8, 8)),
+        dict(m=0, n=1280, k=9 * 2560, conv=(_nb, 8, 8)),
+        dict(m=0, n=320, k=9 * 960, conv=(_nb, 64, 64)),
+    ]
+CASES += [
+    # 3x3 stride 2 (Downsample): dA through the column buffer, dB implicit with TMA element strides
+    dict(m=0, n=320, k=9 * 320, conv=(2, 64, 64), stride=2, bias="row"),
+    dict(m=0, n=640, k=9 * 640, conv=(2, 32, 32), stride=2),
+    dict(m=0, n=1280, k=9 * 1280, conv=(2, 16, 16), stride=2),
+    # a 12x8 latent does not tile into the TMA boxes: column path for dA, im2col for dB
+    dict(m=0, n=320, k=9 * 320, conv=(2, 12, 8), bias="row"),
+    dict(m=0, n=320, k=9 * 320, conv=(2, 12, 8), stride=2),
+]
+
+
+def case_id(kw):
+    return "-".join(f"{k}={v}" for k, v in kw.items()).replace(" ", "").replace("'", "")
