@@ -24,13 +24,6 @@
 
 namespace mdb {
 
-int get_attn_tuning();
-void count_launch(int n = 1);
-void set_attn_tuning(int v);
-
-constexpr int kAttnConsumers = 256;                 // warpgroups 0 and 1
-constexpr int kAttnProducerWarp = kAttnConsumers / 32;
-constexpr int kAttnThreads = kAttnConsumers + 32;
 constexpr int kBQ = 128;
 
 template <int D, int BKV, int STAGES>
@@ -65,15 +58,14 @@ struct AttnLseKParams : AttnKParams {
 // MINB = 2 caps the registers so that two CTAs (four MMA warpgroups) share an SM.  LSE: also store the row
 // log-sum-exp (then the parameters are an AttnLseKParams); without it the kernel is exactly the inference one.
 template <int D, int BKV, int STAGES, int MINB, bool LSE = false>
-__global__ void __launch_bounds__(kAttnThreads, MINB)
+__global__ void __launch_bounds__(kWsThreads, MINB)
     attn_wg_kernel(const __grid_constant__ std::conditional_t<LSE, AttnLseKParams, AttnKParams> p) {
   using C = AttnCfg<D, BKV, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t q_bar;
   __shared__ __align__(8) uint64_t kv_full[STAGES], kv_empty[STAGES];
 
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
+  uint8_t* sQ = align1024(smem_raw);
   uint8_t* sKV = sQ + C::kQBytes;
 
   const int warp = threadIdx.x >> 5;
@@ -86,28 +78,23 @@ __global__ void __launch_bounds__(kAttnThreads, MINB)
   const int n_tiles = t0 + t1;
 
   pdl_launch_dependents();
-  if (warp == kAttnProducerWarp && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK0);
     tma_prefetch_desc(&p.tmV0);
     mbar_init(&q_bar, 1);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], kAttnConsumers);
-    }
+    ring_init<STAGES>(kv_full, kv_empty, 1);
     fence_barrier_init();
   }
   __syncthreads();
   pdl_wait();
 
-  if (warp == kAttnProducerWarp) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       mbar_expect_tx(&q_bar, C::kQBytes);
       for (int dc = 0; dc < C::kDkChunks; ++dc)
         tma_load_3d(sQ + dc * (kBQ * 128), &p.tmQ, &q_bar, dc * 64, head, b * p.nq + q0);
       for (int j = 0; j < n_tiles; ++j) {
-        const int s = j % STAGES;
-        const uint32_t ph = (j / STAGES) & 1;
         const bool src1 = j >= t0;
         const int key0 = (src1 ? (j - t0) : j) * BKV;
         const CUtensorMap* tk = src1 ? &p.tmK1 : &p.tmK0;
@@ -115,7 +102,7 @@ __global__ void __launch_bounds__(kAttnThreads, MINB)
         const int nsrc = src1 ? p.n1 : p.n0;
         const int kvb = src1 ? (p.kv1_batches > 1 ? b : 0) : (p.kv0_batches > 1 ? b : 0);
         const int ldvb = src1 ? p.ldv1_batch : p.ldv0_batch;
-        mbar_wait(&kv_empty[s], ph ^ 1);
+        const int s = ring_acquire<STAGES>(kv_empty, j);
         mbar_expect_tx(&kv_full[s], C::kStageBytes);
         uint8_t* sk = sKV + s * C::kStageBytes;
         uint8_t* sv = sk + C::kKBytes;
@@ -137,11 +124,10 @@ __global__ void __launch_bounds__(kAttnThreads, MINB)
     mbar_wait(&q_bar, 0);
 
     for (int j = 0; j < n_tiles; ++j) {
-      const int s = j % STAGES;
       const bool src1 = j >= t0;
       const int key0 = (src1 ? (j - t0) : j) * BKV;
       const int valid = min(BKV, (src1 ? p.n1 : p.n0) - key0);
-      mbar_wait(&kv_full[s], (j / STAGES) & 1);
+      const int s = ring_wait_full<STAGES>(kv_full, j);
       const uint32_t k_addr = smem_u32(sKV + s * C::kStageBytes);
       const uint32_t v_addr = k_addr + C::kKBytes;
 
@@ -253,13 +239,9 @@ template <int D, int BKV, int STAGES, int MINB, bool LSE = false, typename P>
 static int launch_attn(const P& kp, dim3 grid, cudaStream_t st) {
   using C = AttnCfg<D, BKV, STAGES>;
   static_assert(MINB == 1 || C::kSmem <= 113 * 1024, "two CTAs per SM must fit");
-  static bool attr_set = false;
-  auto kern = attn_wg_kernel<D, BKV, STAGES, MINB, LSE>;
-  if (!attr_set) {
-    MDB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem));
-    attr_set = true;
-  }
-  MDB_CHECK_CUDA(launch_pdl(kern, grid, dim3(kAttnThreads), C::kSmem, st, kp));
+  constexpr auto kern = attn_wg_kernel<D, BKV, STAGES, MINB, LSE>;
+  if (int rc = set_max_dyn_smem<kern>(C::kSmem)) return rc;
+  MDB_CHECK_CUDA(launch_pdl(kern, grid, dim3(kWsThreads), C::kSmem, st, kp));
   count_launch();
   return MDB_OK;
 }
@@ -272,25 +254,14 @@ static int build_and_launch(const mdb_attn_desc* a, float* lse, cudaStream_t st)
   memset(&kp, 0, sizeof(kp));
   const int hd = a->heads * a->d;
   int rc;
-  {
-    uint64_t dims[3] = {(uint64_t)a->d, (uint64_t)a->heads, (uint64_t)a->batch * a->nq};
-    uint64_t str[2] = {(uint64_t)a->d * 2, (uint64_t)a->ldq * 2};
-    uint32_t box[3] = {64, 1, kBQ};
-    if ((rc = make_tmap_f16(&kp.tmQ, a->q, 3, dims, str, box))) return rc;
-  }
+  if ((rc = tmap_heads(&kp.tmQ, a->q, a->d, a->heads, (uint64_t)a->batch * a->nq, a->ldq, kBQ))) return rc;
   auto mk_kv = [&](const void* k, long long ldk, const void* vt, long long ldvt, int n, int nb, int ldvb,
                    CUtensorMap* tk, CUtensorMap* tv) -> int {
-    uint64_t dims[3] = {(uint64_t)a->d, (uint64_t)a->heads, (uint64_t)nb * n};
-    uint64_t str[2] = {(uint64_t)a->d * 2, (uint64_t)ldk * 2};
-    uint32_t box[3] = {64, 1, (uint32_t)BKV};
-    int r = make_tmap_f16(tk, k, 3, dims, str, box);
+    int r = tmap_heads(tk, k, a->d, a->heads, (uint64_t)nb * n, ldk, BKV);
     if (r) return r;
     // kDV rows from row head * d: rows past d (d = 40 -> 48) are the next head's or zero-filled, and only feed
     // output columns >= d, which are never stored
-    uint64_t vdims[2] = {(uint64_t)nb * ldvb, (uint64_t)hd};
-    uint64_t vstr[1] = {(uint64_t)ldvt * 2};
-    uint32_t vbox[2] = {64, (uint32_t)kDV};
-    return make_tmap_f16(tv, vt, 2, vdims, vstr, vbox);
+    return tmap_rows(tv, vt, (uint64_t)nb * ldvb, hd, ldvt, 64, kDV);
   };
   if ((rc = mk_kv(a->k0, a->ldk0, a->vt0, a->ldvt0, a->n0, a->kv0_batches, a->ldv0_batch, &kp.tmK0, &kp.tmV0))) return rc;
   if (a->n1 > 0) {

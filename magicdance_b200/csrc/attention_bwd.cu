@@ -25,12 +25,8 @@
 
 namespace mdb {
 
-void count_launch(int n = 1);
 int attention_check_desc(const mdb_attn_desc* a);
 
-constexpr int kBwdConsumers = 256;  // warpgroups 0 and 1
-constexpr int kBwdProducerWarp = kBwdConsumers / 32;
-constexpr int kBwdThreads = kBwdConsumers + 32;
 constexpr int kBwdRows = 128;  // queries per dQ CTA, keys per dK/dV CTA
 constexpr int kBwdStep = 64;   // keys per dQ step, queries per dK/dV step: one 128-byte swizzle row of V^T
 constexpr float kLog2e = 1.4426950408889634f;
@@ -74,15 +70,11 @@ struct AttnBwdKParams {
   float scale, scale_log2;
 };
 
-__device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
-  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // dQ (and D): one CTA per 128 queries x head x batch element
 // ------------------------------------------------------------------------------------------------------------------
 template <int D>
-__global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_dq_kernel(const __grid_constant__ AttnBwdKParams p) {
+__global__ void __launch_bounds__(kWsThreads, 1) attn_bwd_dq_kernel(const __grid_constant__ AttnBwdKParams p) {
   using C = BwdCfg<D>;
   constexpr int STAGES = C::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -103,18 +95,15 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_dq_kernel(const __gri
   const int n_tiles = t0 + t1;
 
   pdl_launch_dependents();
-  if (warp == kBwdProducerWarp && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     mbar_init(&q_bar, 1);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], kBwdConsumers);
-    }
+    ring_init<STAGES>(kv_full, kv_empty, 1);
     fence_barrier_init();
   }
   __syncthreads();
   pdl_wait();
 
-  if (warp == kBwdProducerWarp) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       mbar_expect_tx(&q_bar, 2 * C::kTile128);
       for (int dc = 0; dc < C::kDkChunks; ++dc)
@@ -124,10 +113,9 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_dq_kernel(const __gri
           tma_load_3d(sDO + dc * C::kChunk128 + half * C::kChunk64, &p.tmDO, &q_bar, dc * 64, head, row);
         }
       for (int j = 0; j < n_tiles; ++j) {
-        const int s = j % STAGES;
         const int src = j >= t0 ? 1 : 0;
         const int key0 = (src ? j - t0 : j) * kBwdStep;
-        mbar_wait(&kv_empty[s], ((j / STAGES) & 1) ^ 1);
+        const int s = ring_acquire<STAGES>(kv_empty, j);
         mbar_expect_tx(&kv_full[s], C::kDqStage);
         uint8_t* sk = sKV + s * C::kDqStage;
         for (int dc = 0; dc < C::kDkChunks; ++dc)
@@ -177,10 +165,9 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_dq_kernel(const __gri
   mbar_wait(&q_bar, 0);
 
   for (int j = 0; j < n_tiles; ++j) {
-    const int s = j % STAGES;
     const int src = j >= t0 ? 1 : 0;
     const int valid = min(kBwdStep, p.n[src] - (src ? j - t0 : j) * kBwdStep);
-    mbar_wait(&kv_full[s], (j / STAGES) & 1);
+    const int s = ring_wait_full<STAGES>(kv_full, j);
     const uint32_t k_addr = kv_base + s * C::kDqStage;
     const uint32_t vt_addr = k_addr + C::kTile64;
 
@@ -243,7 +230,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_dq_kernel(const __gri
 // dK / dV: one CTA per 128 keys of one source x head x batch element.  MODE bit 0: dV, bit 1: dK.
 // ------------------------------------------------------------------------------------------------------------------
 template <int D, int MODE>
-__global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdKParams p) {
+__global__ void __launch_bounds__(kWsThreads, 1) attn_bwd_dkdv_kernel(const __grid_constant__ AttnBwdKParams p) {
   using C = BwdCfg<D>;
   constexpr int STAGES = C::kStages;
   constexpr bool kDV_ = (MODE & 1) != 0, kDK = (MODE & 2) != 0;
@@ -269,18 +256,15 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_dkdv_kernel(const __g
   const long long stat0 = (static_cast<long long>(b) * gridDim.y + head) * p.nq;
 
   pdl_launch_dependents();
-  if (warp == kBwdProducerWarp && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     mbar_init(&kv_bar, 1);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&q_full[s], 32);  // every producer lane arrives after writing its LSE / D entries
-      mbar_init(&q_empty[s], kBwdConsumers);
-    }
+    ring_init<STAGES>(q_full, q_empty, 32);  // every producer lane arrives on q_full after writing its LSE / D entries
     fence_barrier_init();
   }
   __syncthreads();
   pdl_wait();
 
-  if (warp == kBwdProducerWarp) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       mbar_expect_tx(&kv_bar, C::kTile128 + (kDK ? 2 * C::kVtBytes : 0));
       for (int dc = 0; dc < C::kDkChunks; ++dc)
@@ -293,8 +277,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_dkdv_kernel(const __g
                       b * p.ldv_batch[src] + key0 + half * kBwdStep, head * D);
     }
     for (int j = 0; j < n_qt; ++j) {
-      const int s = j % STAGES;
-      mbar_wait(&q_empty[s], ((j / STAGES) & 1) ^ 1);
+      const int s = ring_acquire<STAGES>(q_empty, j);
       for (int c = lane; c < kBwdStep; c += 32) {
         const int q = j * kBwdStep + c;
         s_lse2[s][c] = q < p.nq ? p.lse[stat0 + q] * kLog2e : INFINITY;  // queries past nq: P = 0
@@ -327,8 +310,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_dkdv_kernel(const __g
   mbar_wait(&kv_bar, 0);
 
   for (int j = 0; j < n_qt; ++j) {
-    const int s = j % STAGES;
-    mbar_wait(&q_full[s], (j / STAGES) & 1);
+    const int s = ring_wait_full<STAGES>(q_full, j);
     const uint32_t q_addr = qd_base + s * C::kKvStage;
     // opaque per step: otherwise the loop-invariant K and V^T descriptors of every K step are hoisted out of the
     // loop and held in registers, which spills the d = 160 dK pass
@@ -439,15 +421,6 @@ __global__ void __launch_bounds__(kBwdThreads, 1) attn_bwd_dkdv_kernel(const __g
 // ------------------------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------------------------
-template <typename K>
-static int set_smem(K kern, int bytes, bool* done) {
-  if (!*done) {
-    MDB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-    *done = true;
-  }
-  return MDB_OK;
-}
-
 template <int D>
 static int bwd_launch(const mdb_attn_bwd_desc* a, cudaStream_t st) {
   using C = BwdCfg<D>;
@@ -456,19 +429,14 @@ static int bwd_launch(const mdb_attn_bwd_desc* a, cudaStream_t st) {
   memset(&kp, 0, sizeof(kp));
   const int hd = f->heads * D;
   int rc;
+  // the forward's head slices (attention.cu), 64 tokens per box
   auto mk_rows = [&](CUtensorMap* m, const void* base, long long ld, long long rows) -> int {
-    uint64_t dims[3] = {(uint64_t)D, (uint64_t)f->heads, (uint64_t)rows};
-    uint64_t str[2] = {(uint64_t)D * 2, (uint64_t)ld * 2};
-    uint32_t box[3] = {64, 1, (uint32_t)kBwdStep};
-    return make_tmap_f16(m, base, 3, dims, str, box);
+    return tmap_heads(m, base, D, f->heads, rows, ld, kBwdStep);
   };
+  // kDV rows from row head * d: rows past d (d = 40 -> 48) are the next head's or zero-filled; they meet only the
+  // zero-filled channels d..47 of the dO tile
   auto mk_vt = [&](CUtensorMap* m, const void* base, long long ld, long long cols) -> int {
-    // kDV rows from row head * d: rows past d (d = 40 -> 48) are the next head's or zero-filled; they meet only the
-    // zero-filled channels d..47 of the dO tile
-    uint64_t dims[2] = {(uint64_t)cols, (uint64_t)hd};
-    uint64_t str[1] = {(uint64_t)ld * 2};
-    uint32_t box[2] = {64, (uint32_t)C::kDV};
-    return make_tmap_f16(m, base, 2, dims, str, box);
+    return tmap_rows(m, base, cols, hd, ld, 64, C::kDV);
   };
   if ((rc = mk_rows(&kp.tmQ, f->q, f->ldq, (long long)f->batch * f->nq))) return rc;
   if ((rc = mk_rows(&kp.tmDO, a->dout, a->lddout, (long long)f->batch * f->nq))) return rc;
@@ -504,25 +472,22 @@ static int bwd_launch(const mdb_attn_bwd_desc* a, cudaStream_t st) {
   kp.scale = f->scale;
   kp.scale_log2 = f->scale * kLog2e;
 
-  static bool dq_set = false;
-  if ((rc = set_smem(attn_bwd_dq_kernel<D>, C::kDqSmem, &dq_set))) return rc;
+  if ((rc = set_max_dyn_smem<attn_bwd_dq_kernel<D>>(C::kDqSmem))) return rc;
   const dim3 gq((f->nq + kBwdRows - 1) / kBwdRows, f->heads, f->batch);
-  MDB_CHECK_CUDA(launch_pdl(attn_bwd_dq_kernel<D>, gq, dim3(kBwdThreads), C::kDqSmem, st, kp));
+  MDB_CHECK_CUDA(launch_pdl(attn_bwd_dq_kernel<D>, gq, dim3(kWsThreads), C::kDqSmem, st, kp));
   count_launch();
 
   const int tiles = (f->n0 + kBwdRows - 1) / kBwdRows + (bank ? (f->n1 + kBwdRows - 1) / kBwdRows : 0);
   const dim3 gk(tiles, f->heads, f->batch);
   if constexpr (D == 160) {  // one 64 x 160 accumulator per warpgroup per pass: dV, then dK
-    static bool v_set = false, k_set = false;
-    if ((rc = set_smem(attn_bwd_dkdv_kernel<D, 1>, C::kKvSmem, &v_set))) return rc;
-    if ((rc = set_smem(attn_bwd_dkdv_kernel<D, 2>, C::kKvSmem, &k_set))) return rc;
-    MDB_CHECK_CUDA(launch_pdl(attn_bwd_dkdv_kernel<D, 1>, gk, dim3(kBwdThreads), C::kKvSmem, st, kp));
-    MDB_CHECK_CUDA(launch_pdl(attn_bwd_dkdv_kernel<D, 2>, gk, dim3(kBwdThreads), C::kKvSmem, st, kp));
+    if ((rc = set_max_dyn_smem<attn_bwd_dkdv_kernel<D, 1>>(C::kKvSmem))) return rc;
+    if ((rc = set_max_dyn_smem<attn_bwd_dkdv_kernel<D, 2>>(C::kKvSmem))) return rc;
+    MDB_CHECK_CUDA(launch_pdl(attn_bwd_dkdv_kernel<D, 1>, gk, dim3(kWsThreads), C::kKvSmem, st, kp));
+    MDB_CHECK_CUDA(launch_pdl(attn_bwd_dkdv_kernel<D, 2>, gk, dim3(kWsThreads), C::kKvSmem, st, kp));
     count_launch(2);
   } else {
-    static bool kv_set = false;
-    if ((rc = set_smem(attn_bwd_dkdv_kernel<D, 3>, C::kKvSmem, &kv_set))) return rc;
-    MDB_CHECK_CUDA(launch_pdl(attn_bwd_dkdv_kernel<D, 3>, gk, dim3(kBwdThreads), C::kKvSmem, st, kp));
+    if ((rc = set_max_dyn_smem<attn_bwd_dkdv_kernel<D, 3>>(C::kKvSmem))) return rc;
+    MDB_CHECK_CUDA(launch_pdl(attn_bwd_dkdv_kernel<D, 3>, gk, dim3(kWsThreads), C::kKvSmem, st, kp));
     count_launch();
   }
   return MDB_OK;

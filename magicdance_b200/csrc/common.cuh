@@ -1,5 +1,6 @@
 // Shared device/host helpers for the sm_90a kernels: mbarrier, TMA, cluster and wgmma PTX wrappers,
-// wgmma descriptors, TMA tensor-map construction and error plumbing for the C ABI.
+// the operand ring of the warp-specialised kernels, wgmma descriptors, TMA tensor-map construction
+// and error plumbing for the C ABI.
 #pragma once
 
 #include <cuda.h>
@@ -37,17 +38,36 @@ void set_error(const char* fmt, ...);
     }                               \
   } while (0)
 
+// launch counter behind mdb_launch_count(); launch heuristics behind mdb_set_tuning() / mdb_get_tuning()
+void count_launch(int n = 1);
+int get_gemm_tuning(int key);
+void set_gemm_tuning(int key, int value);
+int get_attn_tuning();
+void set_attn_tuning(int v);
+
+constexpr int kNumSms = 132;  // H100 SXM: the SM count that the grid-size heuristics plan for
+
 // ----------------------------------------------------------------------------------------------
-// TMA tensor maps (host)
+// TMA tensor maps (host): fp16 tiled maps with 128-byte swizzle.  Each returns 0 or an MDB_ERR_* code.
 // ----------------------------------------------------------------------------------------------
-// fp16 tiled map with 128B swizzle; dims[0] is the contiguous dimension; strides_bytes[i] is the
-// byte stride of dims[i+1].  Returns 0 on success.
-int make_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                  const uint64_t* strides_bytes, const uint32_t* box);
-// the same with a chosen swizzle and TMA element strides (nullptr = 1 along every dimension)
-int make_tmap_f16_sw(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                     const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle,
-                     const uint32_t* elem_strides = nullptr);
+// [rows][inner] row-major, `ld` elements between rows; boxes of box_rows x box_inner
+int tmap_rows(CUtensorMap* out, const void* base, uint64_t inner, uint64_t rows, long long ld, uint32_t box_inner,
+              uint32_t box_rows);
+// the head slices of [tokens][heads * d] activations (row stride ld) as (d, heads, tokens); boxes of 64 channels x
+// 1 head x box_tokens tokens, zero-filled beyond d
+int tmap_heads(CUtensorMap* out, const void* base, int d, int heads, uint64_t tokens, long long ld,
+               uint32_t box_tokens);
+// NHWC images [nb][h][w] of pixels `ld` elements apart, c channels used, as (c, w, h, nb); cs = 2 reads every second
+// pixel along w and h (TMA element strides)
+int tmap_nhwc(CUtensorMap* out, const void* base, int c, int w, int h, int nb, long long ld, const uint32_t box[4],
+              int cs);
+
+// The 4-D TMA box {64 channels, x, y, images} that covers `rows` consecutive output pixels of a 3x3 conv with ho x wo
+// output pixels per image, reading every cs-th input pixel.  `fwd` selects the forward kernel's rule for rows at
+// least as wide as the box: only rows strictly wider are cut into single-row boxes, and only at stride 1.  Returns
+// kBoxOk, or the condition that fails (such runs of pixels are then not boxes).
+enum { kBoxOk, kBoxWideRows, kBoxRowsPerTile, kBoxImagesPerTile, kBoxTooLarge };
+int pixel_box(int ho, int wo, int cs, int rows, bool fwd, uint32_t box[4]);
 
 // ----------------------------------------------------------------------------------------------
 // device-side PTX wrappers
@@ -95,6 +115,17 @@ template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
                               Args&&... args) {
   return launch_pdl_cluster2(kernel, grid, block, smem, stream, 1u, 1u, static_cast<Args&&>(args)...);
+}
+// raises the dynamic shared-memory limit of Kernel to `bytes`, once.  The flag belongs to the kernel itself: kernels
+// of the same type (gemm_bwd_kernel<0> and <1>) each get their own.
+template <auto Kernel>
+inline int set_max_dyn_smem(int bytes) {
+  static bool done = false;
+  if (!done) {
+    MDB_CHECK_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    done = true;
+  }
+  return MDB_OK;
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -144,6 +175,41 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "DONE:\n\t}"
       ::"r"(addr), "r"(parity)
       : "memory");
+}
+
+// ---- warp-specialised TMA -> wgmma kernels ------------------------------------------------------
+// Warp roles: warps 0-7 are two MMA warpgroups (the consumers), warp 8 is the TMA producer.
+constexpr int kConsumers = 256;
+constexpr int kProducerWarp = kConsumers / 32;
+constexpr int kWsThreads = kConsumers + 32;
+
+// 128-byte-swizzled TMA tiles and wgmma descriptors need 1024-byte-aligned shared memory
+__device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
+}
+
+// The S-stage operand ring: step `it` uses stage it % S.  The producer fills a stage once its `empty` barrier shows
+// that the consumers released the previous round; the consumers read it once its `full` barrier completes.
+template <int S>
+__device__ __forceinline__ void ring_init(uint64_t* full, uint64_t* empty, uint32_t full_count) {
+  for (int s = 0; s < S; ++s) {
+    mbar_init(&full[s], full_count);
+    mbar_init(&empty[s], kConsumers);  // every consumer thread arrives when it is done with the stage
+  }
+}
+// producer: wait until the stage of step `it` is free and return it (the caller then arms `full` with expect_tx)
+template <int S>
+__device__ __forceinline__ int ring_acquire(uint64_t* empty, int it) {
+  const int s = it % S;
+  mbar_wait(&empty[s], ((it / S) & 1) ^ 1);
+  return s;
+}
+// consumer: wait until the stage of step `it` is loaded and return it
+template <int S>
+__device__ __forceinline__ int ring_wait_full(uint64_t* full, int it) {
+  const int s = it % S;
+  mbar_wait(&full[s], (it / S) & 1);
+  return s;
 }
 
 // ---- TMA loads (global -> shared, completion on an mbarrier) -----------------------------------

@@ -22,14 +22,8 @@
 
 namespace mdb {
 
-int get_gemm_tuning(int key);
-void set_gemm_tuning(int key, int value);
-
 constexpr int kBM = 128;
 constexpr int kBK = 64;  // 64 halves = 128 B = one swizzle row
-constexpr int kGemmConsumers = 256;                   // warpgroups 0 and 1
-constexpr int kProducerWarp = kGemmConsumers / 32;     // warp 8
-constexpr int kGemmThreads = kGemmConsumers + 32;
 
 struct GemmKParams {
   CUtensorMap tmA;
@@ -124,7 +118,7 @@ __device__ __forceinline__ void epi_store_chunk(const GemmKParams& p, long long 
 }
 
 template <int BN, bool GEGLU, int kStages>
-__global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPerSm))
+__global__ void __launch_bounds__(kWsThreads, (GemmSmem<BN, kStages>::kCtasPerSm))
     gemm_tc_kernel(const __grid_constant__ GemmKParams p) {
   using S = GemmSmem<BN, kStages>;
   extern __shared__ uint8_t smem_raw[];
@@ -134,7 +128,7 @@ __global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPer
   __shared__ __align__(16) float s_lnu[BN];   // this N tile's u (LayerNorm folded into the GEMM)
   __shared__ float2 s_ln[kBM];                // (mean, rstd) of each row of the tile (LayerNorm fusion)
 
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = align1024(smem_raw);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * kBM;
@@ -151,20 +145,17 @@ __global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPer
   if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kGemmConsumers);
-    }
+    ring_init<kStages>(full_bar, empty_bar, 1);
     fence_barrier_init();
   }
   // a bias row that serves all batches is a constant weight: stage it before the PDL wait (overlaps the
   // previous kernel's tail).  Per-batch biases (timestep embedding) are produced upstream and are read later.
   const bool bias_in_smem = (p.bias != nullptr) && (p.bias_batch_stride == 0) && !p.cluster_reduce;
   if (bias_in_smem && warp < kProducerWarp) {
-    for (int j = threadIdx.x; j < BN; j += kGemmConsumers) s_bias[j] = (n0 + j < p.n) ? p.bias[n0 + j] : 0.f;
+    for (int j = threadIdx.x; j < BN; j += kConsumers) s_bias[j] = (n0 + j < p.n) ? p.bias[n0 + j] : 0.f;
   }
   if (ln && warp < kProducerWarp) {  // a constant of the weights, like the bias
-    for (int j = threadIdx.x; j < BN; j += kGemmConsumers) s_lnu[j] = (n0 + j < p.n) ? p.ln_u[n0 + j] : 0.f;
+    for (int j = threadIdx.x; j < BN; j += kConsumers) s_lnu[j] = (n0 + j < p.n) ? p.ln_u[n0 + j] : 0.f;
   }
   __syncthreads();
   pdl_wait();  // everything above overlapped the previous kernel's tail; global memory from here on
@@ -179,9 +170,7 @@ __global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPer
         x0 = (p.hw >= kBM) ? (m0 % p.hw) % p.w : 0;  // != 0 only for rows wider than the 128-pixel tile
       }
       for (int it = 0; it < n_iter; ++it) {
-        const int s = it % kStages;
-        const uint32_t ph = (it / kStages) & 1;
-        mbar_wait(&empty_bar[s], ph ^ 1);
+        const int s = ring_acquire<kStages>(empty_bar, it);
         uint8_t* sa = smem + s * S::kStageBytes;
         uint8_t* sb = sa + S::kABytes;
         const int kc = kc_begin + it;
@@ -202,7 +191,7 @@ __global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPer
   } else {
     // ---------------- warpgroups 0, 1: main loop on wgmma, then the epilogue ----------------
     const int wg = warp >> 2;          // this warpgroup's 64 rows of the tile
-    const int tid = threadIdx.x;       // 0 .. kGemmConsumers-1
+    const int tid = threadIdx.x;       // 0 .. kConsumers-1
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -212,8 +201,7 @@ __global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPer
     const int ln_row = tid >> 1, ln_half = tid & 1;
     float pivot = 0.f, ls0 = 0.f, ls1 = 0.f, lq0 = 0.f, lq1 = 0.f;
     for (int it = 0; it < n_iter; ++it) {
-      const int s = it % kStages;
-      mbar_wait(&full_bar[s], (it / kStages) & 1);
+      const int s = ring_wait_full<kStages>(full_bar, it);
       const uint32_t a_addr = smem_u32(smem + s * S::kStageBytes);
       const uint64_t da = wgmma_desc_k_sw128(a_addr + wg * (64 * 128));
       const uint64_t db = wgmma_desc_k_sw128(a_addr + S::kABytes);
@@ -260,7 +248,7 @@ __global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPer
     }
     // Both warpgroups' MMAs are complete, so the operand ring is idle: park the fp32 tile in it, [128][kRedLd]
     // (the layout the split-K cluster reduction reads), and run the epilogue with one thread per row.
-    named_bar_sync(1, kGemmConsumers);
+    named_bar_sync(1, kConsumers);
     float* red = reinterpret_cast<float*>(smem);
     {
       const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -271,7 +259,7 @@ __global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPer
         *reinterpret_cast<float2*>(red + row_t * kRedLd + col) = make_float2(acc[j], acc[j + 1]);
       }
     }
-    named_bar_sync(1, kGemmConsumers);
+    named_bar_sync(1, kConsumers);
 
     const int rt = tid & (kBM - 1);   // row inside the tile
     const int half = tid / kBM;       // which of the tile's column chunks this thread takes (alternating)
@@ -383,7 +371,7 @@ __global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPer
       if (p.residual != nullptr) {
 #pragma unroll
         for (int q = 0; q < kMaxItems; ++q) {
-          const int item = threadIdx.x + q * kGemmThreads;
+          const int item = threadIdx.x + q * kWsThreads;
           if (item < R * groups) {
             const int rl = item / groups, cgp = item - rl * groups;
             const long long row = static_cast<long long>(m0) + static_cast<int>(crank) * R + rl;
@@ -395,8 +383,8 @@ __global__ void __launch_bounds__(kGemmThreads, (GemmSmem<BN, kStages>::kCtasPer
       cluster_sync_all();
       const uint32_t red_base = smem_u32(smem);
 #pragma unroll 1
-      for (int it_ = 0; it_ * kGemmThreads < R * groups; ++it_) {
-        const int item = threadIdx.x + it_ * kGemmThreads;
+      for (int it_ = 0; it_ * kWsThreads < R * groups; ++it_) {
+        const int item = threadIdx.x + it_ * kWsThreads;
         if (item >= R * groups) break;
         const int rl = item / groups, cgp = item - rl * groups;
         const int rt = static_cast<int>(crank) * R + rl;  // row inside the tile
@@ -509,77 +497,36 @@ __global__ void splitk_finalize_kernel(GemmKParams p) {
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
-
-int make_tmap_f16_sw(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                     const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle,
-                     const uint32_t* elem_strides) {
-  if (g_encode == nullptr) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
-    if (e != cudaSuccess || fn == nullptr || qres != cudaDriverEntryPointSuccess) {
-      set_error("cuTensorMapEncodeTiled not available from the driver (%s)", cudaGetErrorString(e));
-      return MDB_ERR_CUDA;
-    }
-    g_encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+int pixel_box(int ho, int wo, int cs, int rows, bool fwd, uint32_t box[4]) {
+  const int hw = ho * wo;
+  if (fwd ? wo > rows : wo >= rows) {
+    // rows as wide as the tile or wider (the VAE's 256- and 512-pixel levels): `rows` consecutive pixels of ONE row
+    if (wo % rows || (fwd && cs != 1)) return kBoxWideRows;
+    box[1] = cs * rows; box[2] = 1; box[3] = 1;
+  } else if (hw >= rows) {
+    if (rows % wo || hw % rows) return kBoxRowsPerTile;
+    box[1] = cs * wo; box[2] = cs * (rows / wo); box[3] = 1;
+  } else {
+    if (rows % hw) return kBoxImagesPerTile;
+    box[1] = cs * wo; box[2] = cs * ho; box[3] = rows / hw;
   }
-  cuuint64_t gdim[5];
-  cuuint64_t gstr[4];
-  cuuint32_t bx[5];
-  cuuint32_t es[5];
-  for (int i = 0; i < rank; ++i) {
-    gdim[i] = dims[i];
-    bx[i] = box[i];
-    es[i] = elem_strides ? elem_strides[i] : 1;
-    if (i > 0) gstr[i - 1] = strides_bytes[i - 1];
-  }
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) {
-    set_error("TMA base address %p is not 16-byte aligned", base);
-    return MDB_ERR_INVALID;
-  }
-  for (int i = 0; i + 1 < rank; ++i) {
-    if (gstr[i] % 16 != 0) {
-      set_error("TMA stride %d (%llu bytes) is not a multiple of 16", i, (unsigned long long)gstr[i]);
-      return MDB_ERR_INVALID;
-    }
-  }
-  CUresult r = g_encode(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(base), gdim, gstr, bx, es,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed with CUresult %d (rank %d, dims %llu,%llu box %u,%u)", (int)r, rank,
-              (unsigned long long)gdim[0], (unsigned long long)(rank > 1 ? gdim[1] : 0), bx[0], rank > 1 ? bx[1] : 0);
-    return MDB_ERR_CUDA;
-  }
-  return MDB_OK;
+  box[0] = 64;
+  return box[1] <= 256 && box[2] <= 256 ? kBoxOk : kBoxTooLarge;
 }
-
-int make_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                  const uint32_t* box) {
-  return make_tmap_f16_sw(out, base, rank, dims, strides_bytes, box, CU_TENSOR_MAP_SWIZZLE_128B);
-}
-
-void count_launch(int n = 1);
 
 // launch heuristics (mdb_set_tuning)
 static int g_pair_min_tiles = 128;  // smallest grid, in 128-row tile equivalents, that goes to the 256-wide tiles
 static int g_bn80_below = 100;      // N % 160 == 0 layers with fewer 160-wide CTAs than this use 80-wide tiles
 constexpr int kLongKChunks = 64;    // ... unless K >= 4096 (automatic split-K): then 160-wide tiles and split K
-constexpr int kSms = 132;           // H100 SXM
 
 template <int BN, bool GEGLU, int STAGES>
 static int launch_gemm(const GemmKParams& kp, dim3 grid, cudaStream_t st) {
   const unsigned cluster_z = kp.cluster_reduce ? static_cast<unsigned>(kp.splits) : 1u;
-  static bool attr_set = false;
-  auto kern = gemm_tc_kernel<BN, GEGLU, STAGES>;
+  constexpr auto kern = gemm_tc_kernel<BN, GEGLU, STAGES>;
   constexpr int kSmem = GemmSmem<BN, STAGES>::kTotal;
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
-  if (!attr_set) {
-    MDB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    attr_set = true;
-  }
-  MDB_CHECK_CUDA(launch_pdl_cluster(kern, grid, dim3(kGemmThreads), kSmem, st, cluster_z, kp));
+  if (int rc = set_max_dyn_smem<kern>(kSmem)) return rc;
+  MDB_CHECK_CUDA(launch_pdl_cluster(kern, grid, dim3(kWsThreads), kSmem, st, cluster_z, kp));
   count_launch();
   return MDB_OK;
 }
@@ -646,23 +593,12 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
     MDB_REQUIRE(g->m == g->nb * ho * wo, "mdb_gemm_f16: conv m != nb*ho*wo");
     const int hw = ho * wo;  // OUTPUT pixels per image: tiles are cut over these
     uint32_t box[4];
-    if (wo > kBM) {
-      // rows wider than the tile (the VAE's 256- and 512-pixel levels): a tile is 128 consecutive pixels of ONE row
-      MDB_REQUIRE(wo % kBM == 0 && cs == 1, "mdb_gemm_f16: conv rows wider than 128 pixels need 128 | w and stride 1 (w=%d)", g->w);
-      box[0] = kBK; box[1] = kBM; box[2] = 1; box[3] = 1;
-    } else if (hw >= kBM) {
-      MDB_REQUIRE(kBM % wo == 0 && hw % kBM == 0,
-                  "mdb_gemm_f16: conv tile needs w | 128 and 128 | h*w (output h=%d w=%d)", ho, wo);
-      box[0] = kBK; box[1] = cs * wo; box[2] = cs * (kBM / wo); box[3] = 1;
-    } else {
-      MDB_REQUIRE(kBM % hw == 0, "mdb_gemm_f16: conv tile needs h*w | 128 (output h=%d w=%d)", ho, wo);
-      box[0] = kBK; box[1] = cs * wo; box[2] = cs * ho; box[3] = kBM / hw;
-    }
-    MDB_REQUIRE(box[1] <= 256 && box[2] <= 256, "mdb_gemm_f16: conv TMA box too large");
-    uint64_t dims[4] = {(uint64_t)g->c, (uint64_t)g->w, (uint64_t)g->h, (uint64_t)g->nb};
-    uint64_t str[3] = {(uint64_t)g->c * 2, (uint64_t)g->c * g->w * 2, (uint64_t)g->c * g->h * g->w * 2};
-    const uint32_t estr[4] = {1u, (uint32_t)cs, (uint32_t)cs, 1u};
-    rc = make_tmap_f16_sw(&kp.tmA, g->a, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, cs == 2 ? estr : nullptr);
+    const int why = pixel_box(ho, wo, cs, kBM, true, box);
+    MDB_REQUIRE(why != kBoxWideRows, "mdb_gemm_f16: conv rows wider than 128 pixels need 128 | w and stride 1 (w=%d)", g->w);
+    MDB_REQUIRE(why != kBoxRowsPerTile, "mdb_gemm_f16: conv tile needs w | 128 and 128 | h*w (output h=%d w=%d)", ho, wo);
+    MDB_REQUIRE(why != kBoxImagesPerTile, "mdb_gemm_f16: conv tile needs h*w | 128 (output h=%d w=%d)", ho, wo);
+    MDB_REQUIRE(why != kBoxTooLarge, "mdb_gemm_f16: conv TMA box too large");
+    rc = tmap_nhwc(&kp.tmA, g->a, g->c, g->w, g->h, g->nb, g->c, box, cs);
     if (rc) return rc;
     kp.chunks_per_tap = g->c / kBK;
     kp.w = wo;
@@ -672,15 +608,10 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
   } else {
     const int k1 = g->a2 ? g->k1 : g->k;
     MDB_REQUIRE(k1 % kBK == 0 && k1 > 0 && k1 <= g->k, "mdb_gemm_f16: k1=%d must be a multiple of 64 within K", k1);
-    uint32_t box[2] = {kBK, kBM};
-    uint64_t dims[2] = {(uint64_t)k1, (uint64_t)g->m};
-    uint64_t str[1] = {(uint64_t)g->lda * 2};
-    rc = make_tmap_f16(&kp.tmA, g->a, 2, dims, str, box);
+    rc = tmap_rows(&kp.tmA, g->a, k1, g->m, g->lda, kBK, kBM);
     if (rc) return rc;
     if (g->a2) {
-      uint64_t dims2[2] = {(uint64_t)(g->k - k1), (uint64_t)g->m};
-      uint64_t str2[1] = {(uint64_t)g->lda2 * 2};
-      rc = make_tmap_f16(&kp.tmA2, g->a2, 2, dims2, str2, box);
+      rc = tmap_rows(&kp.tmA2, g->a2, g->k - k1, g->m, g->lda2, kBK, kBM);
       if (rc) return rc;
     }
     kp.k1_chunks = k1 / kBK;
@@ -713,18 +644,13 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
     // the weight-streaming 3x3 convs of the 8x8 ... 32x32 levels at one frame) keep the wide tile and split K —
     // see the automatic split-K below (scripts/gpu_microbench.py times the tile width x split-K choices)
     const long long tiles160 = (long long)m_tiles * (g->n / 160) * (g->splits > 1 ? g->splits : 1);
-    const bool wide_split = g->splits == 0 && kp.k_chunks >= kLongKChunks && tiles160 * 2 <= kSms;
+    const bool wide_split = g->splits == 0 && kp.k_chunks >= kLongKChunks && tiles160 * 2 <= kNumSms;
     bn = (tiles160 < g_bn80_below && !wide_split) ? 80 : 160;
   } else {
     bn = 128;
   }
-  {
-    uint32_t box[2] = {kBK, (uint32_t)bn};
-    uint64_t dims[2] = {(uint64_t)g->k, (uint64_t)g->n};
-    uint64_t str[1] = {(uint64_t)g->ldb * 2};
-    rc = make_tmap_f16(&kp.tmB, g->b, 2, dims, str, box);
-    if (rc) return rc;
-  }
+  rc = tmap_rows(&kp.tmB, g->b, g->k, g->n, g->ldb, kBK, bn);
+  if (rc) return rc;
 
   int splits = g->splits > 1 ? g->splits : 1;
   if (g->ln_u != nullptr) splits = 1;  // the correction is applied by the CTA that holds the whole K range
@@ -735,7 +661,7 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
     const long long tiles = (long long)m_tiles * ((g->n + bn - 1) / bn);
     if (tiles < 100)
       for (int c = 8; c >= 2; c >>= 1)
-        if (tiles * c <= kSms && kp.k_chunks / c >= 16) {
+        if (tiles * c <= kNumSms && kp.k_chunks / c >= 16) {
           splits = c;
           break;
         }
@@ -754,7 +680,7 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
   }
 
   dim3 grid(m_tiles, (g->n + bn - 1) / bn, splits);
-  const bool deep = (long long)grid.x * grid.y * grid.z <= kSms && kp.chunks_per_split >= 12;
+  const bool deep = (long long)grid.x * grid.y * grid.z <= kNumSms && kp.chunks_per_split >= 12;
   if (pair) {
     if (bn == 256) rc = geglu ? launch_gemm<256, true, 4>(kp, grid, st) : launch_gemm<256, false, 4>(kp, grid, st);
     else if (bn == 160) rc = launch_gemm<160, false, 6>(kp, grid, st);
@@ -769,7 +695,7 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
   if (splits > 1 && !kp.cluster_reduce) {
     const long long total = ((long long)g->m * g->n + 3) / 4;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > kSms * 8) blocks = kSms * 8;
+    if (blocks > kNumSms * 8) blocks = kNumSms * 8;
     MDB_CHECK_CUDA(launch_pdl(splitk_finalize_kernel, dim3(blocks), dim3(256), 0, st, kp));
     count_launch();
   }

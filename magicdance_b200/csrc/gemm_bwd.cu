@@ -20,25 +20,16 @@
 // a fixed order, no scatter-add); dB for such latents through im2col + the plain path.
 #include "common.cuh"
 
-extern "C" int mdb_im2col3x3_f16(const void* x, void* col, int32_t batch, int32_t h, int32_t w, int32_t c,
-                                 int32_t stride, mdb_stream_t stream);
-
 namespace mdb {
-
-void count_launch(int n = 1);
 
 constexpr int kGbM = 128;  // output rows per CTA
 constexpr int kGbN = 128;  // output columns per CTA
 constexpr int kGbK = 64;   // reduction step per stage: one 128-byte swizzle row
 constexpr int kGbStages = 3;
-constexpr int kGbConsumers = 256;
-constexpr int kGbProducerWarp = kGbConsumers / 32;
-constexpr int kGbThreads = kGbConsumers + 32;
 constexpr int kGbABytes = kGbM * kGbK * 2;    // 16 KB
 constexpr int kGbChunk = 64 * kGbK * 2;       // 8 KB: 64 output rows or columns x 64 reduction steps
 constexpr int kGbStageBytes = kGbABytes + (kGbN / 64) * kGbChunk;
 constexpr int kGbSmem = kGbStages * kGbStageBytes + 1024;  // two CTAs per SM
-constexpr int kGbSms = 132;
 constexpr int kBiasRows = 256;  // rows per partial column sum
 
 struct GbOut {  // a gradient destination: fp16 or fp32 rows, overwritten or accumulated into; p == nullptr: dropped
@@ -90,11 +81,11 @@ __device__ __forceinline__ void gb_put(const GemmBwdKParams& p, long long row, i
 }
 
 template <int TA>
-__global__ void __launch_bounds__(kGbThreads, 2) gemm_bwd_kernel(const __grid_constant__ GemmBwdKParams p) {
+__global__ void __launch_bounds__(kWsThreads, 2) gemm_bwd_kernel(const __grid_constant__ GemmBwdKParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kGbStages];
   __shared__ __align__(8) uint64_t empty_bar[kGbStages];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = align1024(smem_raw);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int r0 = blockIdx.x * kGbM;
@@ -107,17 +98,14 @@ __global__ void __launch_bounds__(kGbThreads, 2) gemm_bwd_kernel(const __grid_co
   const int b_chunks = min(kGbN / 64, (p.cols - c0) / 64);
 
   pdl_launch_dependents();
-  if (warp == kGbProducerWarp && lane == 0) {
-    for (int s = 0; s < kGbStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kGbConsumers);
-    }
+  if (warp == kProducerWarp && lane == 0) {
+    ring_init<kGbStages>(full_bar, empty_bar, 1);
     fence_barrier_init();
   }
   __syncthreads();
   pdl_wait();
 
-  if (warp == kGbProducerWarp) {
+  if (warp == kProducerWarp) {
     if (lane == 0 && n_iter > 0) {
       int b0 = 0, y0 = 0, x0 = 0;  // TA = 0 conv: the first pixel of this row tile
       if (TA == 0 && p.conv) {
@@ -126,8 +114,7 @@ __global__ void __launch_bounds__(kGbThreads, 2) gemm_bwd_kernel(const __grid_co
         x0 = (r0 - b0 * p.hw) - y0 * p.w;
       }
       for (int it = 0; it < n_iter; ++it) {
-        const int s = it % kGbStages;
-        mbar_wait(&empty_bar[s], ((it / kGbStages) & 1) ^ 1);
+        const int s = ring_acquire<kGbStages>(empty_bar, it);
         uint8_t* sa = smem + s * kGbStageBytes;
         uint8_t* sb = sa + kGbABytes;
         const int kc = kc_begin + it;
@@ -174,8 +161,7 @@ __global__ void __launch_bounds__(kGbThreads, 2) gemm_bwd_kernel(const __grid_co
 #pragma unroll
   for (int i = 0; i < kGbN / 2; ++i) acc[i] = 0.f;
   for (int it = 0; it < n_iter; ++it) {
-    const int s = it % kGbStages;
-    mbar_wait(&full_bar[s], (it / kGbStages) & 1);
+    const int s = ring_wait_full<kGbStages>(full_bar, it);
     const uint32_t a_addr = smem_u32(smem + s * kGbStageBytes) + wg * kGbChunk;  // this warpgroup's 64 rows
     const uint32_t b_addr = smem_u32(smem + s * kGbStageBytes) + kGbABytes;
     wgmma_fence();
@@ -303,24 +289,6 @@ __global__ void colsum_finalize_kernel(const float* ws, int n, int segs, int par
 // ------------------------------------------------------------------------------------------------------------------
 // host
 // ------------------------------------------------------------------------------------------------------------------
-// The 4-D TMA box (channels, x, y, images) that covers `rows` consecutive output pixels of images with ho x wo output
-// pixels, reading every cs-th input pixel; false when such runs of pixels are not boxes (then the column path runs).
-static bool pixel_box(int ho, int wo, int cs, int rows, uint32_t box[4]) {
-  const int hw = ho * wo;
-  if (wo >= rows) {
-    if (wo % rows) return false;
-    box[1] = cs * rows; box[2] = 1; box[3] = 1;
-  } else if (hw >= rows) {
-    if (rows % wo || hw % rows) return false;
-    box[1] = cs * wo; box[2] = cs * (rows / wo); box[3] = 1;
-  } else {
-    if (rows % hw) return false;
-    box[1] = cs * wo; box[2] = cs * ho; box[3] = rows / hw;
-  }
-  box[0] = 64;
-  return box[1] <= 256 && box[2] <= 256;
-}
-
 struct GbPlan {
   bool da, db, dbias;
   int m, cs, ho, wo;
@@ -335,7 +303,7 @@ struct GbPlan {
 static void pick_splits(int requested, long long tiles, int chunks, int* splits, int* cps) {
   int s = requested;
   if (s <= 0) {  // automatic: about two CTAs per SM, every split keeps at least 8 chunks (512 rows of the reduction)
-    s = static_cast<int>(2 * kGbSms / tiles);
+    s = static_cast<int>(2 * kNumSms / tiles);
     s = min(s, chunks / 8);
     s = min(s, 16);
   }
@@ -384,9 +352,10 @@ static int plan_bwd(const mdb_gemm_bwd_desc* g, GbPlan* pl) {
     pl->wo = (f->w - 1) / pl->cs + 1;
     MDB_REQUIRE(f->m == f->nb * pl->ho * pl->wo, "mdb_gemm_bwd_f16: conv m != nb*ho*wo");
     if (pl->da) MDB_REQUIRE(g->da != nullptr && g->da2 == nullptr, "mdb_gemm_bwd_f16: conv dA goes to da only");
+    // pixels that do not form TMA boxes take the column path
     uint32_t box[4];
-    pl->da_col = pl->cs == 2 || !pixel_box(f->h, f->w, 1, kGbM, box);
-    pl->db_col = !pixel_box(pl->ho, pl->wo, pl->cs, 64, box);
+    pl->da_col = pl->cs == 2 || pixel_box(f->h, f->w, 1, kGbM, false, box) != kBoxOk;
+    pl->db_col = pixel_box(pl->ho, pl->wo, pl->cs, 64, false, box) != kBoxOk;
   } else {
     const int k1 = f->a2 ? f->k1 : f->k;
     MDB_REQUIRE(k1 % 64 == 0 && k1 > 0 && k1 <= f->k, "mdb_gemm_bwd_f16: k1=%d must be a multiple of 64 within K", k1);
@@ -428,24 +397,18 @@ static int launch_bwd_gemm(int ta, GemmBwdKParams& kp, int tiles_x, int splits, 
   kp.splits = splits;
   kp.chunks_per_split = cps;
   const dim3 grid(tiles_x, (kp.cols + kGbN - 1) / kGbN, splits);
-  static bool attr0 = false, attr1 = false;
+  int rc;
   if (ta == 0) {
-    if (!attr0) {
-      MDB_CHECK_CUDA(cudaFuncSetAttribute(gemm_bwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGbSmem));
-      attr0 = true;
-    }
-    MDB_CHECK_CUDA(launch_pdl(gemm_bwd_kernel<0>, grid, dim3(kGbThreads), kGbSmem, st, kp));
+    if ((rc = set_max_dyn_smem<gemm_bwd_kernel<0>>(kGbSmem))) return rc;
+    MDB_CHECK_CUDA(launch_pdl(gemm_bwd_kernel<0>, grid, dim3(kWsThreads), kGbSmem, st, kp));
   } else {
-    if (!attr1) {
-      MDB_CHECK_CUDA(cudaFuncSetAttribute(gemm_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGbSmem));
-      attr1 = true;
-    }
-    MDB_CHECK_CUDA(launch_pdl(gemm_bwd_kernel<1>, grid, dim3(kGbThreads), kGbSmem, st, kp));
+    if ((rc = set_max_dyn_smem<gemm_bwd_kernel<1>>(kGbSmem))) return rc;
+    MDB_CHECK_CUDA(launch_pdl(gemm_bwd_kernel<1>, grid, dim3(kWsThreads), kGbSmem, st, kp));
   }
   count_launch();
   if (splits > 1) {
     const long long pairs = static_cast<long long>(kp.rows) * kp.cols / 2;
-    const int blocks = static_cast<int>(min((pairs + 255) / 256, static_cast<long long>(kGbSms) * 8));
+    const int blocks = static_cast<int>(min((pairs + 255) / 256, static_cast<long long>(kNumSms) * 8));
     MDB_CHECK_CUDA(launch_pdl(gemm_bwd_finalize_kernel, dim3(blocks), dim3(256), 0, st, kp));
     count_launch();
   }
@@ -466,20 +429,14 @@ static int run_da(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st)
   GemmBwdKParams kp;
   memset(&kp, 0, sizeof(kp));
   int rc;
-  {  // the forward's B [N][K]: 64 columns x 64 rows (the reduction) per box, read MN-major
-    uint64_t dims[2] = {(uint64_t)f->k, (uint64_t)f->n};
-    uint64_t str[1] = {(uint64_t)f->ldb * 2};
-    uint32_t box[2] = {64, 64};
-    if ((rc = make_tmap_f16(&kp.tmB, f->b, 2, dims, str, box))) return rc;
-  }
+  // the forward's B [N][K]: 64 columns x 64 rows (the reduction) per box, read MN-major
+  if ((rc = tmap_rows(&kp.tmB, f->b, f->k, f->n, f->ldb, 64, 64))) return rc;
   kp.cols = f->k;
   int tiles_x;
   if (f->conv && !pl.da_col) {  // stride 1, implicit: the row tiles are input pixels
     uint32_t box[4];
-    pixel_box(f->h, f->w, 1, kGbM, box);
-    uint64_t dims[4] = {(uint64_t)f->n, (uint64_t)f->w, (uint64_t)f->h, (uint64_t)f->nb};
-    uint64_t str[3] = {(uint64_t)g->lddd * 2, (uint64_t)g->lddd * f->w * 2, (uint64_t)g->lddd * f->h * f->w * 2};
-    if ((rc = make_tmap_f16_sw(&kp.tmD, g->dd, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    pixel_box(f->h, f->w, 1, kGbM, false, box);
+    if ((rc = tmap_nhwc(&kp.tmD, g->dd, f->n, f->w, f->h, f->nb, g->lddd, box, 1))) return rc;
     kp.conv = 1;
     kp.chunks_per_tap = (f->n + 63) / 64;
     kp.chunks = 9 * kp.chunks_per_tap;
@@ -492,10 +449,7 @@ static int run_da(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st)
     kp.out[0] = gb_out(g->da, g->ldda, g->da_dtype, g->da_accumulate);
     kp.split_col = f->c;
   } else {
-    uint64_t dims[2] = {(uint64_t)f->n, (uint64_t)f->m};
-    uint64_t str[1] = {(uint64_t)g->lddd * 2};
-    uint32_t box[2] = {64, kGbM};
-    if ((rc = make_tmap_f16(&kp.tmD, g->dd, 2, dims, str, box))) return rc;
+    if ((rc = tmap_rows(&kp.tmD, g->dd, f->n, f->m, g->lddd, 64, kGbM))) return rc;
     kp.chunks = (f->n + 63) / 64;
     kp.rows = f->m;
     if (pl.da_col) {
@@ -512,7 +466,7 @@ static int run_da(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st)
   if ((rc = launch_bwd_gemm(0, kp, tiles_x, pl.da_splits, pl.da_cps, st))) return rc;
   if (pl.da_col) {
     const long long total = static_cast<long long>(f->nb) * f->h * f->w * (f->c / 2);
-    const int blocks = static_cast<int>(min((total + 255) / 256, static_cast<long long>(kGbSms) * 16));
+    const int blocks = static_cast<int>(min((total + 255) / 256, static_cast<long long>(kNumSms) * 16));
     MDB_CHECK_CUDA(launch_pdl(col2im_gather_kernel, dim3(blocks), dim3(256), 0, st, static_cast<const float*>(g->ws),
                               gb_out(g->da, g->ldda, g->da_dtype, g->da_accumulate), f->nb, f->h, f->w, f->c, pl.cs,
                               pl.ho, pl.wo));
@@ -526,20 +480,12 @@ static int run_db(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st)
   GemmBwdKParams kp;
   memset(&kp, 0, sizeof(kp));
   int rc;
-  {  // dD^T: 64 of N x 64 of M per box, read MN-major
-    uint64_t dims[2] = {(uint64_t)f->n, (uint64_t)f->m};
-    uint64_t str[1] = {(uint64_t)g->lddd * 2};
-    uint32_t box[2] = {64, 64};
-    if ((rc = make_tmap_f16(&kp.tmD, g->dd, 2, dims, str, box))) return rc;
-  }
-  uint32_t box2[2] = {64, 64};
+  // dD^T: 64 of N x 64 of M per box, read MN-major
+  if ((rc = tmap_rows(&kp.tmD, g->dd, f->n, f->m, g->lddd, 64, 64))) return rc;
   if (f->conv && !pl.db_col) {  // the forward's shifted pixel boxes, 64 output pixels x 64 channels of one tap
     uint32_t box[4];
-    pixel_box(pl.ho, pl.wo, pl.cs, 64, box);
-    uint64_t dims[4] = {(uint64_t)f->c, (uint64_t)f->w, (uint64_t)f->h, (uint64_t)f->nb};
-    uint64_t str[3] = {(uint64_t)f->c * 2, (uint64_t)f->c * f->w * 2, (uint64_t)f->c * f->h * f->w * 2};
-    const uint32_t estr[4] = {1u, (uint32_t)pl.cs, (uint32_t)pl.cs, 1u};
-    if ((rc = make_tmap_f16_sw(&kp.tmB, f->a, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, estr))) return rc;
+    pixel_box(pl.ho, pl.wo, pl.cs, 64, false, box);
+    if ((rc = tmap_nhwc(&kp.tmB, f->a, f->c, f->w, f->h, f->nb, f->c, box, pl.cs))) return rc;
     kp.conv = 1;
     kp.c = f->c;
     kp.w = pl.wo;
@@ -547,20 +493,12 @@ static int run_db(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st)
     kp.cs = pl.cs;
   } else if (f->conv) {  // latents that do not tile: im2col into the workspace, then the plain path
     if ((rc = mdb_im2col3x3_f16(f->a, g->ws, f->nb, f->h, f->w, f->c, pl.cs, st))) return rc;
-    uint64_t dims[2] = {(uint64_t)f->k, (uint64_t)f->m};
-    uint64_t str[1] = {(uint64_t)f->k * 2};
-    if ((rc = make_tmap_f16(&kp.tmB, g->ws, 2, dims, str, box2))) return rc;
+    if ((rc = tmap_rows(&kp.tmB, g->ws, f->k, f->m, f->k, 64, 64))) return rc;
     kp.k1 = f->k;
   } else {
     const int k1 = f->a2 ? f->k1 : f->k;
-    uint64_t dims[2] = {(uint64_t)k1, (uint64_t)f->m};
-    uint64_t str[1] = {(uint64_t)f->lda * 2};
-    if ((rc = make_tmap_f16(&kp.tmB, f->a, 2, dims, str, box2))) return rc;
-    if (f->a2) {
-      uint64_t dims2[2] = {(uint64_t)(f->k - k1), (uint64_t)f->m};
-      uint64_t str2[1] = {(uint64_t)f->lda2 * 2};
-      if ((rc = make_tmap_f16(&kp.tmB2, f->a2, 2, dims2, str2, box2))) return rc;
-    }
+    if ((rc = tmap_rows(&kp.tmB, f->a, k1, f->m, f->lda, 64, 64))) return rc;
+    if (f->a2 && (rc = tmap_rows(&kp.tmB2, f->a2, f->k - k1, f->m, f->lda2, 64, 64))) return rc;
     kp.k1 = k1;
   }
   kp.rows = f->n;

@@ -22,9 +22,79 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
-void count_launch(int n = 1);
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 bool pdl_enabled() { return true; }  // every launch carries the programmatic-stream-serialization attribute
+
+static PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
+
+// fp16 tiled map with 128B swizzle; dims[0] is the contiguous dimension; strides_bytes[i] is the byte stride of
+// dims[i+1]; elem_strides: TMA element strides (nullptr = 1 along every dimension)
+static int make_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                         const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* elem_strides = nullptr) {
+  if (g_encode == nullptr) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
+    if (e != cudaSuccess || fn == nullptr || qres != cudaDriverEntryPointSuccess) {
+      set_error("cuTensorMapEncodeTiled not available from the driver (%s)", cudaGetErrorString(e));
+      return MDB_ERR_CUDA;
+    }
+    g_encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+  }
+  cuuint64_t gdim[5];
+  cuuint64_t gstr[4];
+  cuuint32_t bx[5];
+  cuuint32_t es[5];
+  for (int i = 0; i < rank; ++i) {
+    gdim[i] = dims[i];
+    bx[i] = box[i];
+    es[i] = elem_strides ? elem_strides[i] : 1;
+    if (i > 0) gstr[i - 1] = strides_bytes[i - 1];
+  }
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) {
+    set_error("TMA base address %p is not 16-byte aligned", base);
+    return MDB_ERR_INVALID;
+  }
+  for (int i = 0; i + 1 < rank; ++i) {
+    if (gstr[i] % 16 != 0) {
+      set_error("TMA stride %d (%llu bytes) is not a multiple of 16", i, (unsigned long long)gstr[i]);
+      return MDB_ERR_INVALID;
+    }
+  }
+  CUresult r = g_encode(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(base), gdim, gstr, bx, es,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed with CUresult %d (rank %d, dims %llu,%llu box %u,%u)", (int)r, rank,
+              (unsigned long long)gdim[0], (unsigned long long)(rank > 1 ? gdim[1] : 0), bx[0], rank > 1 ? bx[1] : 0);
+    return MDB_ERR_CUDA;
+  }
+  return MDB_OK;
+}
+
+int tmap_rows(CUtensorMap* out, const void* base, uint64_t inner, uint64_t rows, long long ld, uint32_t box_inner,
+              uint32_t box_rows) {
+  const uint64_t dims[2] = {inner, rows};
+  const uint64_t str[1] = {(uint64_t)ld * 2};
+  const uint32_t box[2] = {box_inner, box_rows};
+  return make_tmap_f16(out, base, 2, dims, str, box);
+}
+
+int tmap_heads(CUtensorMap* out, const void* base, int d, int heads, uint64_t tokens, long long ld,
+               uint32_t box_tokens) {
+  const uint64_t dims[3] = {(uint64_t)d, (uint64_t)heads, tokens};
+  const uint64_t str[2] = {(uint64_t)d * 2, (uint64_t)ld * 2};
+  const uint32_t box[3] = {64, 1, box_tokens};
+  return make_tmap_f16(out, base, 3, dims, str, box);
+}
+
+int tmap_nhwc(CUtensorMap* out, const void* base, int c, int w, int h, int nb, long long ld, const uint32_t box[4],
+              int cs) {
+  const uint64_t dims[4] = {(uint64_t)c, (uint64_t)w, (uint64_t)h, (uint64_t)nb};
+  const uint64_t str[3] = {(uint64_t)ld * 2, (uint64_t)ld * w * 2, (uint64_t)ld * h * w * 2};
+  const uint32_t estr[4] = {1u, (uint32_t)cs, (uint32_t)cs, 1u};
+  return make_tmap_f16(out, base, 4, dims, str, box, cs == 2 ? estr : nullptr);
+}
 
 // ---------------------------------------------------------------------------------------------
 // direct 3x3 conv, pad 1, stride 1|2, NHWC fp16, fp32 accumulate.
@@ -455,7 +525,7 @@ __global__ void cfg_ddim_update_kernel(float* x, const float* __restrict__ ec, c
 }
 
 
-static inline int grid_for(long long total, int threads = 256, int cap = 132 * 16) {
+static inline int grid_for(long long total, int threads = 256, int cap = kNumSms * 16) {
   long long b = (total + threads - 1) / threads;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
@@ -465,13 +535,6 @@ static inline int grid_for(long long total, int threads = 256, int cap = 132 * 1
 }  // namespace mdb
 
 using namespace mdb;
-
-namespace mdb {
-int get_gemm_tuning(int key);
-void set_gemm_tuning(int key, int value);
-int get_attn_tuning();
-void set_attn_tuning(int v);
-}  // namespace mdb
 
 extern "C" int mdb_abi_version(void) { return MDB_ABI_VERSION; }
 
@@ -613,12 +676,8 @@ extern "C" int mdb_conv3x3_direct_f16(const void* x, const void* wt, const float
   const long long npix = static_cast<long long>(batch) * h * w;
   if (stride == 1 && cin == 4 && cout % 8 == 0 && cout * 36 * 4 <= 96 * 1024 && kCiSlots * (cout / 8) <= kCiMaxThreads) {
     // tiny-cin path (input conv)
-    static bool attr_set = false;
     const int smem = cout * 36 * 4;
-    if (!attr_set) {
-      MDB_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_smallcin_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-      attr_set = true;
-    }
+    if (int rc = set_max_dyn_smem<conv3x3_smallcin_kernel<4>>(96 * 1024)) return rc;
     const int threads = ((kCiSlots * (cout / 8) + 31) / 32) * 32;
     const int per_block = kCiSlots * kCiPixPerThread;
     MDB_CHECK_CUDA(launch_pdl(conv3x3_smallcin_kernel<4>, dim3(static_cast<unsigned>((npix + per_block - 1) / per_block)),
@@ -630,14 +689,10 @@ extern "C" int mdb_conv3x3_direct_f16(const void* x, const void* wt, const float
   }
   if (stride == 1 && cout == 4 && cin % 8 == 0 && residual == nullptr && cout * 9 * cin * 2 <= 96 * 1024) {
     // tiny-cout path (output conv)
-    static bool attr_set = false;
     const int smem = cout * 9 * cin * 2;
-    if (!attr_set) {
-      MDB_CHECK_CUDA(cudaFuncSetAttribute(conv3x3_smallcout_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-      attr_set = true;
-    }
+    if (int rc = set_max_dyn_smem<conv3x3_smallcout_kernel<4>>(96 * 1024)) return rc;
     int blocks = static_cast<int>((npix + 7) / 8);
-    if (blocks > 132 * 4) blocks = 132 * 4;
+    if (blocks > kNumSms * 4) blocks = kNumSms * 4;
     MDB_CHECK_CUDA(launch_pdl(conv3x3_smallcout_kernel<4>, dim3(blocks), dim3(256), smem, st,
                               static_cast<const __half*>(x), static_cast<const __half*>(wt), bias,
                               static_cast<__half*>(y), batch, h, w, cin, silu));

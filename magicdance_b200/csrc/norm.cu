@@ -19,8 +19,6 @@
 
 namespace mdb {
 
-void count_launch(int n = 1);
-
 __device__ __forceinline__ const uint4* gn_src(const __half* x1, int c1, const __half* x2, int c2, long long row,
                                                 int ch) {
   // channel ch (multiple of 8) of concatenated row -> address of its 16-byte vector
@@ -399,7 +397,7 @@ extern "C" int mdb_groupnorm_f16(const void* x1, int32_t c1, const void* x2, int
   if (gn_use_cluster(c, c1, c2, batch, mode)) {
     // cluster size: enough CTAs to cover the SMs about twice, at least ~64 pixels per CTA, at most 8 (portable)
     int cs = 1;
-    while (cs < 8 && 32 * batch * cs * 2 <= 2 * 132 && hw / (cs * 2) >= 64) cs *= 2;  // 132 SMs
+    while (cs < 8 && 32 * batch * cs * 2 <= 2 * kNumSms && hw / (cs * 2) >= 64) cs *= 2;
     MDB_CHECK_CUDA(launch_pdl_cluster(gn_cluster_kernel, dim3(32, batch, cs), dim3(kGnFusedThreads), 0, st,
                                       static_cast<unsigned>(cs), static_cast<const __half*>(x1), c1,
                                       static_cast<const __half*>(x2), c2, gamma, beta, static_cast<__half*>(y), hw, eps,

@@ -120,6 +120,37 @@ def _workspace(key, numel, dtype, device, zero=False):
     return t
 
 
+def _gemm_m(a, conv, conv_stride, m):
+    """rows of D: the output pixels of the 3x3 pad-1 conv, else m (default: a's rows)"""
+    if conv is not None:
+        nb, h, wd, _ = conv
+        return nb * ((h - 1) // conv_stride + 1) * ((wd - 1) // conv_stride + 1)
+    return a.shape[0] if m is None else m
+
+
+def _fill_fwd_desc(g, a, w, a2, conv, conv_stride, m):
+    """fills the A-side fields (a, a2, conv geometry) and m, n, k of the forward GemmDesc g; returns (m, k1)"""
+    n, k = w.shape
+    if conv is not None:
+        nb, h, wd, c = conv
+        assert conv_stride in (1, 2) and a.is_contiguous() and a.numel() == nb * h * wd * c
+        g.conv, g.nb, g.h, g.w, g.c = conv_stride, nb, h, wd, c  # descriptor: conv = 1 (stride 1) | 2 (stride 2)
+        g.a, g.lda, g.k1 = a.data_ptr(), c, k
+    else:
+        assert a.dim() == 2 and a.stride(1) == 1
+        g.a, g.lda, g.k1 = a.data_ptr(), a.stride(0), a.shape[1]
+        if a2 is not None:
+            _chk(a2, torch.float16, "a2")
+            assert a2.dim() == 2 and a2.stride(1) == 1 and a2.shape[0] == a.shape[0]
+            g.a2, g.lda2 = a2.data_ptr(), a2.stride(0)
+            assert a.shape[1] + a2.shape[1] == k
+        else:
+            assert a.shape[1] == k, (a.shape, w.shape)
+    m = _gemm_m(a, conv, conv_stride, m)
+    g.m, g.n, g.k = m, n, k
+    return m, g.k1
+
+
 def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, residual=None, epilogue=EPI_NONE,
          a2=None, conv=None, conv_stride=1, splits=0, m=None, ln_u=None, ln_eps=1e-5):
     """D = epilogue(A @ W^T).  a: [M, K1] fp16 (last dim contiguous, row stride arbitrary) or, with
@@ -133,23 +164,7 @@ def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, re
     _chk(w, torch.float16, "w")
     g = _lib.GemmDesc()
     n, k = w.shape
-    if conv is not None:
-        nb, h, wd, c = conv
-        assert conv_stride in (1, 2) and a.is_contiguous() and a.numel() == nb * h * wd * c
-        m = nb * ((h - 1) // conv_stride + 1) * ((wd - 1) // conv_stride + 1)  # output pixels (3x3, pad 1)
-        g.conv, g.nb, g.h, g.w, g.c = conv_stride, nb, h, wd, c  # descriptor: conv = 1 (stride 1) | 2 (stride 2)
-        g.a, g.lda, g.k1 = a.data_ptr(), c, k
-    else:
-        assert a.dim() == 2 and a.stride(1) == 1
-        m = a.shape[0] if m is None else m
-        g.a, g.lda, g.k1 = a.data_ptr(), a.stride(0), a.shape[1]
-        if a2 is not None:
-            _chk(a2, torch.float16, "a2")
-            assert a2.dim() == 2 and a2.stride(1) == 1 and a2.shape[0] == a.shape[0]
-            g.a2, g.lda2 = a2.data_ptr(), a2.stride(0)
-            assert a.shape[1] + a2.shape[1] == k
-        else:
-            assert a.shape[1] == k, (a.shape, w.shape)
+    m, _ = _fill_fwd_desc(g, a, w, a2, conv, conv_stride, m)
     n_out = n // 2 if epilogue == EPI_GEGLU else n
     if out is None:
         out = torch.empty((m, n_out), dtype=torch.float16, device=a.device)
@@ -165,7 +180,7 @@ def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, re
         _chk(residual, torch.float16, "residual")
         assert residual.dim() == 2 and residual.stride(1) == 1
         g.residual, g.ldr = residual.data_ptr(), residual.stride(0)
-    g.m, g.n, g.k, g.epilogue = m, n, k, epilogue
+    g.epilogue = epilogue
     if ln_u is not None:
         _chk(ln_u, torch.float32, "ln_u")
         assert conv is None and a2 is None and ln_u.numel() == n and ln_u.is_contiguous()
@@ -224,28 +239,11 @@ def gemm_backward(a, w, dd, *, a2=None, conv=None, conv_stride=1, bias_batch_str
     g = _lib.GemmBwdDesc()
     f = g.fwd
     n, k = w.shape
-    if conv is not None:
-        nb, h, wd, c = conv
-        assert conv_stride in (1, 2) and a.is_contiguous() and a.numel() == nb * h * wd * c
-        m = nb * ((h - 1) // conv_stride + 1) * ((wd - 1) // conv_stride + 1)
-        f.conv, f.nb, f.h, f.w, f.c = conv_stride, nb, h, wd, c
-        f.a, f.lda, f.k1 = a.data_ptr(), c, k
-        da_shape, k1 = (nb * h * wd, c), k
-    else:
-        assert a.dim() == 2 and a.stride(1) == 1
-        m = a.shape[0] if m is None else m
-        k1 = a.shape[1]
-        f.a, f.lda, f.k1 = a.data_ptr(), a.stride(0), k1
-        if a2 is not None:
-            _chk(a2, torch.float16, "a2")
-            assert a2.dim() == 2 and a2.stride(1) == 1 and a2.shape[0] == a.shape[0] and k1 + a2.shape[1] == k
-            f.a2, f.lda2 = a2.data_ptr(), a2.stride(0)
-        else:
-            assert k1 == k, (a.shape, w.shape)
-        da_shape = (m, k1)
+    m, k1 = _fill_fwd_desc(f, a, w, a2, conv, conv_stride, m)
+    da_shape = (conv[0] * conv[1] * conv[2], conv[3]) if conv is not None else (m, k1)
     assert w.stride(1) == 1 and dd.shape[0] >= m and dd.shape[1] == n, (dd.shape, m, n)
     f.b, f.ldb = w.data_ptr(), w.stride(0)
-    f.m, f.n, f.k, f.epilogue, f.splits = m, n, k, epilogue, splits
+    f.epilogue, f.splits = epilogue, splits
     f.bias_batch_stride, f.rows_per_batch = bias_batch_stride, rows_per_batch
     if ln_u is not None:
         f.ln_u = ln_u.data_ptr()
@@ -295,10 +293,7 @@ class TcGemm(torch.autograd.Function):
     def forward(ctx, a, a_param, w, w_param, bias, residual, a2, bias_batch_stride, rows_per_batch, conv, conv_stride,
                 splits, m):
         n = w.shape[0]
-        if conv is not None:
-            mm = conv[0] * ((conv[1] - 1) // conv_stride + 1) * ((conv[2] - 1) // conv_stride + 1)
-        else:
-            mm = a.shape[0] if m is None else m
+        mm = _gemm_m(a, conv, conv_stride, m)
         out = torch.empty((mm, (n + 7) // 8 * 8), dtype=torch.float16, device=a.device)[:, :n]
         gemm(a, w, out=out, bias=bias, bias_batch_stride=bias_batch_stride, rows_per_batch=rows_per_batch,
              residual=residual, a2=a2, conv=conv, conv_stride=conv_stride, splits=splits, m=m)
