@@ -18,7 +18,7 @@ from .. import ops
 from ..engine import DenoiseEngine
 from .ddpm import LatentDiffusionReferenceOnly
 from .modules import UNetModel
-from .util import instantiate_from_config
+from .util import _one, instantiate_from_config
 
 
 def _tokens_to_nchw(data, b, h, w):
@@ -108,14 +108,11 @@ class ControlLDMReferenceOnlyPose(LatentDiffusionReferenceOnly):
         """cldm.py:1099-1117 — same arguments, returns eps (B,4,h,w) fp32."""
         assert isinstance(cond, dict)
         assert not self.only_mid_control
-        # a one-element list (every released script) is passed on as the caller's tensor: the engine caches the text
-        # keys/values per tensor identity, and torch.cat would hand it a fresh copy on every call
-        one = lambda lst: lst[0] if len(lst) == 1 else torch.cat(lst, 1)
-        cond_txt = one(cond["c_crossattn"])
+        cond_txt = _one(cond["c_crossattn"])
         if self.control_enabled and cond.get("c_crossattn_void") is not None:
             raise NotImplementedError("c_crossattn_void is never passed by the MagicPose scripts")
         assert self.control_enabled and cond.get("c_concat") is not None, "the pose map (c_concat) is required"
-        cond_hint = one(cond["c_concat"])
+        cond_hint = _one(cond["c_concat"])
         eng = self.engine(x_noisy.device)
         return eng.apply_model(x_noisy, t, cond_txt, cond_hint, reference_image_noisy, uc=uc)
 

@@ -14,7 +14,9 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from ..engine import tensor_key
 from ..pipeline import DenoisePipeline, ddim_parameters, ddim_timesteps_uniform
+from .util import _one
 
 
 class DDIMSampler_ReferenceOnly(object):
@@ -123,8 +125,7 @@ class DDIMSampler_ReferenceOnly(object):
                 and uc.get("image_control") is None and scale != 1.0 and not c.get("overlap_sampling")
                 and not np.any(self.ddim_sigmas) and img.is_cuda):
             return None
-        one = lambda lst: lst[0] if len(lst) == 1 else torch.cat(lst, 1)
-        ref, ctx, pose_map = one(c["image_control"]), one(c["c_crossattn"]), one(c["c_concat"])
+        ref, ctx, pose_map = _one(c["image_control"]), _one(c["c_crossattn"]), _one(c["c_concat"])
         if not (self._rows_identical(ref) and self._rows_identical(ctx)):
             return None  # one reference image and one prompt per batch only (the scripts repeat them per sample)
         pipe = self._pipeline(scale)
@@ -164,9 +165,7 @@ class DDIMSampler_ReferenceOnly(object):
                 group=group, chunk=gd.bank_chunk, storage=ent["storage"])
             ent["ref"] = ref_dev.clone()
         bank = ent["bank"]
-        gd.hint.copy_(pipe.hint(pose_map.to(pipe.device),
-                                frame_key=(pose_map.data_ptr(), pose_map._version, tuple(pose_map.shape)),
-                                keep_alive=pose_map))
+        gd.hint.copy_(pipe.hint(pose_map.to(pipe.device), frame_key=tensor_key(pose_map), keep_alive=pose_map))
         gd.x.copy_(img.to(device=pipe.device, dtype=torch.float32))
         for i in range(total):
             index = total - i - 1
@@ -189,10 +188,9 @@ class DDIMSampler_ReferenceOnly(object):
         from .. import ops
         pipe = self._pipeline(scale)
         dev = pipe.device
-        one = lambda lst: lst[0] if len(lst) == 1 else torch.cat(lst, 1)
-        ref = one(c["image_control"]).to(dev)
+        ref = _one(c["image_control"]).to(dev)
         ref_n = ref if c["wonoise"] else self.model.q_sample(ref, t.to(dev))
-        pair = lambda k: torch.cat([one(uc[k]).to(dev), one(c[k]).to(dev)])
+        pair = lambda k: torch.cat([_one(uc[k]).to(dev), _one(c[k]).to(dev)])
         x = x.to(device=dev, dtype=torch.float32).contiguous()
         cond_in = {"c_concat": [pair("c_concat")], "c_crossattn": [pair("c_crossattn")]}
         eps = self.model.apply_model(torch.cat([x, x]), torch.cat([t, t]).to(dev), cond_in, torch.cat([ref_n, ref_n]))
@@ -206,7 +204,7 @@ class DDIMSampler_ReferenceOnly(object):
         if t.shape[0] == 1:
             return True
         cache = self.model.__dict__.setdefault("_mdb_rows_identical", {})
-        key = (t.untyped_storage().data_ptr(), t.storage_offset(), tuple(t.shape), tuple(t.stride()), t._version)
+        key = tensor_key(t)
         hit = cache.get(key)
         if hit is None:
             if len(cache) >= 8:
@@ -240,27 +238,16 @@ class DDIMSampler_ReferenceOnly(object):
         pipe = self._pipeline(unconditional_guidance_scale)
         dev = pipe.device
         x = x.to(device=dev, dtype=torch.float32)
-        # one-element lists (every released script) are used as they are: torch.cat would hand the engine a fresh
-        # copy every step, and the caches below are keyed on tensor identity
-        one = lambda lst: lst[0] if len(lst) == 1 else torch.cat(lst, 1)
-        ref, ctx, pose_map = one(c["image_control"]), one(c["c_crossattn"]), one(c["c_concat"])
-        if c["wonoise"]:
-            # the clean reference latent feeds the appearance net (ddim.py:532-533): the bank depends on
-            # (reference, t) only.  One reference for the whole batch (the scripts repeat it per sample) is
-            # computed once and broadcast in-kernel; the result is cached per timestep for the next frames.
-            src = c["image_control"][0] if len(c["image_control"]) == 1 else ref
-            shared = self._rows_identical(src) and self._rows_identical(ctx)
-            if shared:
-                bank_kv = pipe.reference_bank(src, ctx, index, first_only=True)
-            else:
-                tt = pipe.t_dev[index].expand(ref.shape[0]).contiguous()
-                bank_kv = pipe.engine.project_bank(pipe.engine.appearance_write(ref, tt, ctx), ref.shape[0])
-        else:  # noised reference (ddim.py:535): depends on fresh noise, cannot be cached
-            ref_n = self.model.q_sample(ref, t.to(ref.device))
-            tt = pipe.t_dev[index].expand(ref.shape[0]).contiguous()
-            bank_kv = pipe.engine.project_bank(pipe.engine.appearance_write(ref_n, tt, ctx), ref.shape[0])
-        hint = pipe.hint(pose_map.to(dev), frame_key=(pose_map.data_ptr(), pose_map._version, tuple(pose_map.shape)),
-                         keep_alive=pose_map)
+        ref, ctx, pose_map = _one(c["image_control"]), _one(c["c_crossattn"]), _one(c["c_concat"])
+        # the clean reference latent feeds the appearance net (ddim.py:532-533): the bank depends on (reference, t)
+        # only.  One reference for the whole batch (the scripts repeat it per sample) is computed once and broadcast
+        # in-kernel; the result is cached per timestep for the next frames.
+        if c["wonoise"] and self._rows_identical(ref) and self._rows_identical(ctx):
+            bank_kv = pipe.reference_bank(ref, ctx, index, first_only=True)
+        else:  # per-sample references, or a noised one (ddim.py:535), which depends on fresh noise: not cached
+            ref_in = ref if c["wonoise"] else self.model.q_sample(ref, t.to(ref.device))
+            bank_kv = pipe.engine.bank_kv(ref_in, pipe.t_dev[index].expand(ref.shape[0]).contiguous(), ctx)
+        hint = pipe.hint(pose_map.to(dev), frame_key=tensor_key(pose_map), keep_alive=pose_map)
         noise = None
         if float(self.ddim_sigmas[index]) != 0.0:
             noise = torch.randn_like(x)

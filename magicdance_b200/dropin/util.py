@@ -57,6 +57,13 @@ def create_model(config_path):
     return model
 
 
+def _one(lst):
+    """a conditioning list as one tensor (torch.cat over channels).  A one-element list (every released script) is
+    passed on as the caller's tensor: the engine caches per tensor identity, and a fresh copy would miss every call."""
+    import torch
+    return lst[0] if len(lst) == 1 else torch.cat(lst, 1)
+
+
 def get_state_dict(container):
     """a checkpoint file holds either the parameter dict itself or {'state_dict': parameter dict, ...}"""
     inner = container.get("state_dict") if isinstance(container, dict) else None

@@ -258,15 +258,23 @@ class Act:
         return self.h * self.w
 
 
+def tensor_key(t):
+    """identity of a tensor's contents as far as the host can tell without a device sync: storage address, view
+    geometry and the in-place version counter.  A cache keyed on it must hold a strong reference to the tensor, so
+    that its storage cannot be freed and the address recycled by another tensor while the entry exists."""
+    return (t.untyped_storage().data_ptr(), t.storage_offset(), tuple(t.shape), tuple(t.stride()), t._version)
+
+
 _warned_sizes = set()
 
 
 def _igemm_ok(h, w, c):
-    """does an h x w x c activation tile into the implicit-GEMM conv's 128-pixel TMA boxes?  (512x512 and 256x256
+    """does an h x w x c conv output tile into the implicit-GEMM conv's 128-pixel TMA boxes?  (512x512 and 256x256
     images do at every level.)  Other sizes work through im2col + GEMM — 9x the activation traffic — so say so once."""
     hw = h * w
     if c % 64:
         return False
+    # mirrors pixel_box(..., fwd=true) in csrc/gemm.cu
     ok = ((128 % w == 0 and hw % 128 == 0) or w % 128 == 0) if hw >= 128 else (128 % hw == 0)
     if not ok and (h, w) not in _warned_sizes:
         _warned_sizes.add((h, w))
@@ -274,6 +282,28 @@ def _igemm_ok(h, w, c):
         warnings.warn(f"magicdance_b200: a {h}x{w} feature map does not tile into 128-pixel TMA boxes; its 3x3 convs take "
                       "the slower im2col + GEMM path (latents whose width divides 128 avoid this)", stacklevel=3)
     return ok
+
+
+def conv3x3(x: Act, w, bias, *, cout, stride=1, residual=None, bias_batch_stride=0) -> Act:
+    """3x3 pad-1 conv, w packed by pack_conv3x3.  Tensor cores (implicit GEMM, else im2col + GEMM) when cin and cout
+    fit their tiles; the direct conv otherwise (few channels in or out: the UNet's conv_in/out, the VAE's ends)."""
+    cin = x.c
+    ho, wo = (x.h - 1) // stride + 1, (x.w - 1) // stride + 1
+    tc = cout % 8 == 0 and cout >= 64 and cin % 64 == 0
+    if tc and _igemm_ok(ho, wo, cin):  # stride 2: TMA element strides of 2, no im2col buffer
+        y = ops.gemm(x.data, w, bias=bias, bias_batch_stride=bias_batch_stride, rows_per_batch=ho * wo,
+                     residual=residual, conv=(x.b, x.h, x.w, cin), conv_stride=stride)
+    elif tc:
+        # latent sizes whose rows do not tile into 128-pixel TMA boxes (e.g. 96x64 -> 12x8 at the deepest
+        # level): explicit im2col + the same tensor-core GEMM
+        col = ops.im2col3x3(x.data, batch=x.b, h=x.h, w=x.w, c=cin, stride=stride)
+        y = ops.gemm(col, w, bias=bias, bias_batch_stride=bias_batch_stride, rows_per_batch=ho * wo,
+                     residual=residual)
+    else:
+        assert bias_batch_stride == 0
+        y = ops.conv3x3_direct(x.data, w, bias, batch=x.b, h=x.h, w=x.w, cin=cin, cout=cout, stride=stride,
+                               residual=residual)
+    return Act(y, x.b, ho, wo)
 
 
 class _BankComplete(Exception):
@@ -315,10 +345,13 @@ class DenoiseEngine:
         e = ops.skinny_linear(e, net.te2_w, net.te2_b)
         return ops.skinny_linear(e, net.emb_w, net.emb_b, silu_in=True)
 
-    def context_kv(self, net: PackedNet, ctx16: torch.Tensor, key):
+    def context_kv(self, net: PackedNet, ctx16: torch.Tensor, context: torch.Tensor, paired=False):
         """Text keys/values of every attn2 (CrossAttention.to_k/to_v on the CLIP context,
-        attention.py:172-174); depends only on the context -> cached per (net, context)."""
-        ck = (id(net),) + tuple(key[:3])  # per PackedNet object: drop-in modules all have an empty key prefix
+        attention.py:172-174); depends only on the context -> cached per (net, context).  ctx16 is the caller's
+        `context` in fp16 on the device, stacked twice when `paired` (the cond | uncond batch of unet_forward)."""
+        # (net, storage, offset, shape, stride, version, paired); per PackedNet object: drop-in modules all have an
+        # empty key prefix
+        ck = (id(net),) + tensor_key(context) + (paired,)
         hit = self._ctx_cache.get(ck)
         if hit is not None:  # the entry's strong reference keeps that storage alive, so the address is still its own
             return hit[0]
@@ -337,27 +370,8 @@ class DenoiseEngine:
             res.append((k, vt, n, b, ldv))
         if len(self._ctx_cache) > 8:
             self._ctx_cache.clear()
-        self._ctx_cache[ck] = (res, key[3] if len(key) > 3 else None)  # strong ref to the context tensor
+        self._ctx_cache[ck] = (res, context)  # strong ref to the context tensor
         return res
-
-    # ---- blocks -------------------------------------------------------------------------------
-    def _conv3(self, x: Act, w, bias, *, cout, residual=None, bias_batch_stride=0):
-        cin = x.c
-        if _igemm_ok(x.h, x.w, cin) and cout % 8 == 0 and cout >= 64:
-            m = x.b * x.hw
-            y = ops.gemm(x.data, w, bias=bias, bias_batch_stride=bias_batch_stride, rows_per_batch=x.hw,
-                         residual=residual, conv=(x.b, x.h, x.w, cin))
-        elif cin % 64 == 0 and cout % 8 == 0 and cout >= 64:
-            # latent sizes whose rows do not tile into 128-pixel TMA boxes (e.g. 96x64 -> 12x8 at the deepest
-            # level): explicit im2col + the same tensor-core GEMM
-            m = x.b * x.hw
-            col = ops.im2col3x3(x.data, batch=x.b, h=x.h, w=x.w, c=cin, stride=1)
-            y = ops.gemm(col, w, bias=bias, bias_batch_stride=bias_batch_stride, rows_per_batch=x.hw,
-                         residual=residual)
-        else:
-            assert bias_batch_stride == 0
-            y = ops.conv3x3_direct(x.data, w, bias, batch=x.b, h=x.h, w=x.w, cin=cin, cout=cout, residual=residual)
-        return Act(y, x.b, x.h, x.w)
 
     # ---- optional intra-network concurrency ---------------------------------------------------------
     # At one or two samples per launch most kernels fill a fraction of the SMs, so independent branches of a
@@ -378,25 +392,24 @@ class DenoiseEngine:
             out = fn()
         return out, (lambda: main.wait_stream(stream))
 
+    # ---- blocks -------------------------------------------------------------------------------
     def _res(self, r: ResW, x: Act, skip: Act | None, emb_all):
         x2 = None if skip is None else skip.data
         if r.skip_w is None:
             assert skip is None
             res, join = x.data, (lambda: None)
         else:
-            m = x.b * x.hw
             res, join = self._fork(lambda: ops.gemm(x.data, r.skip_w, bias=r.skip_b, a2=x2))
         h = ops.groupnorm(x.data, *r.gn1, batch=x.b, hw=x.hw, eps=1e-5, silu=True, x2=x2)
         bias = emb_all[:, r.emb_off:r.emb_off + r.cout]
-        h = self._conv3(Act(h, x.b, x.h, x.w), r.w1, bias, cout=r.cout,
-                        bias_batch_stride=emb_all.stride(0) if emb_all.shape[0] > 1 else 0)
+        h = conv3x3(Act(h, x.b, x.h, x.w), r.w1, bias, cout=r.cout,
+                    bias_batch_stride=emb_all.stride(0) if emb_all.shape[0] > 1 else 0)
         h2 = ops.groupnorm(h.data, *r.gn2, batch=x.b, hw=x.hw, eps=1e-5, silu=True)
         join()
-        return self._conv3(Act(h2, x.b, x.h, x.w), r.w2, r.b2, cout=r.cout, residual=res)
+        return conv3x3(Act(h2, x.b, x.h, x.w), r.w2, r.b2, cout=r.cout, residual=res)
 
     def _transformer(self, a: AttnW, x: Act, ctx_kv, mode, bank, bank_kv, bank_batches):
         b, n, c = x.b, x.hw, a.c
-        m = b * n
         h = ops.groupnorm(x.data, *a.gn, batch=b, hw=n, eps=1e-6, silu=False)
         h = ops.gemm(h, a.pin_w, bias=a.pin_b)
         # --- attn1 (self / self + bank) ---
@@ -436,7 +449,7 @@ class DenoiseEngine:
             p = f"{bp}{j}."
             lw = net.layers[p]
             if kind == "conv_in":
-                x = self._conv3(x, lw[0], lw[1], cout=cout, residual=state.get("hint"))
+                x = conv3x3(x, lw[0], lw[1], cout=cout, residual=state.get("hint"))
             elif kind == "res":
                 x = self._res(lw, x, skip, emb_all)
                 skip = None
@@ -447,16 +460,10 @@ class DenoiseEngine:
                                       state.get("bank_batches", 0))
                 state["attn_i"] = i + 1
             elif kind == "down":
-                ho, wo = (x.h - 1) // 2 + 1, (x.w - 1) // 2 + 1
-                if _igemm_ok(ho, wo, x.c):  # stride-2 implicit GEMM: TMA element strides of 2, no im2col buffer
-                    y = ops.gemm(x.data, lw[0], bias=lw[1], conv=(x.b, x.h, x.w, x.c), conv_stride=2)
-                else:
-                    col = ops.im2col3x3(x.data, batch=x.b, h=x.h, w=x.w, c=x.c, stride=2)
-                    y = ops.gemm(col, lw[0], bias=lw[1])
-                x = Act(y, x.b, ho, wo)
+                x = conv3x3(x, lw[0], lw[1], cout=cout, stride=2)
             elif kind == "up":
                 up = ops.upsample2x(x.data, batch=x.b, h=x.h, w=x.w, c=x.c)
-                x = self._conv3(Act(up, x.b, 2 * x.h, 2 * x.w), lw[0], lw[1], cout=cout)
+                x = conv3x3(Act(up, x.b, 2 * x.h, 2 * x.w), lw[0], lw[1], cout=cout)
         return x
 
     # ---- the three networks -------------------------------------------------------------------
@@ -465,20 +472,15 @@ class DenoiseEngine:
         b, c, h, w = x.shape
         act = Act(ops.nchw_f32_to_nhwc_f16(x, copies=copies), copies * b, h, w)
         ctx16 = context.to(device=self.device, dtype=torch.float16).contiguous()
-        # cache key: storage address + view geometry + version counter (in-place edits invalidate).  The cache
-        # entry holds a strong reference to the tensor, so the storage cannot be freed and its address recycled
-        # by a different context while the entry exists.
-        key = ((context.untyped_storage().data_ptr(), context.storage_offset(), tuple(context.stride())),
-               context._version, tuple(context.shape), context)
-        return act, ctx16, key
+        return act, ctx16
 
     def appearance_write(self, ref_latent, t, context):
         """ControlNetReferenceOnly.forward 'write' (cldm.py:469-497): returns the bank, a list of 16
         norm1(x) token matrices [B*N_l, C_l] fp16 (attention.py:287-298).  Layers after the last
         norm1 (dead compute in the reference, SURVEY §8a a4) are skipped."""
         net = self.appearance
-        x, ctx16, key = self._prep(ref_latent, context)
-        ctx_kvs = self.context_kv(net, ctx16, key)
+        x, ctx16 = self._prep(ref_latent, context)
+        ctx_kvs = self.context_kv(net, ctx16, context)
         emb_all = self.time_bias(net, t, x.b)
         n_total = len(net.attn_layers())
         # in write mode `bank_batches` carries the number of bank entries after which the pass may stop
@@ -531,6 +533,10 @@ class DenoiseEngine:
             res.append((k1, vt1, rows // batches, batches))
         return res
 
+    def bank_kv(self, ref_latent, t, context):
+        """project_bank of the appearance bank of ref_latent: the bank_kv argument of unet_forward"""
+        return self.project_bank(self.appearance_write(ref_latent, t, context), ref_latent.shape[0])
+
     def hint_features(self, pose_map):
         """ControlNet.input_hint_block (cldm.py:599-615); depends only on the pose map."""
         net = self.pose
@@ -552,8 +558,8 @@ class DenoiseEngine:
         emb_all: precomputed time_bias(self.pose, t) (it depends on the timestep only: a sampler computes it once
         per schedule entry instead of once per frame-step)."""
         net = self.pose
-        x, ctx16, key = self._prep(x_noisy, context)
-        ctx_kvs = self.context_kv(net, ctx16, key)
+        x, ctx16 = self._prep(x_noisy, context)
+        ctx_kvs = self.context_kv(net, ctx16, context)
         if emb_all is None:
             emb_all = self.time_bias(net, t, x.b)
         state = {"mode": "plain", "attn_i": 0, "hint": hint_feat}
@@ -579,14 +585,13 @@ class DenoiseEngine:
         layer streams its weights once and sees twice the rows; samples [0,B) read the bank and take the
         pose residuals, samples [B,2B) do neither.  Returns (eps_cond, eps_uncond)."""
         net = self.unet
-        x, ctx16, key = self._prep(x_noisy, context, copies=2 if cfg_pair else 1)
+        x, ctx16 = self._prep(x_noisy, context, copies=2 if cfg_pair else 1)
         b = x_noisy.shape[0]
-        if cfg_pair:
-            assert not uc
-            if ctx16.shape[0] > 1:
-                ctx16 = torch.cat([ctx16, ctx16])
-                key = (key[0], key[1], key[2] + ("pair",), key[3])
-        ctx_kvs = self.context_kv(net, ctx16, key)
+        assert not (cfg_pair and uc)
+        paired = cfg_pair and ctx16.shape[0] > 1  # a single context row is broadcast to both halves as it is
+        if paired:
+            ctx16 = torch.cat([ctx16, ctx16])
+        ctx_kvs = self.context_kv(net, ctx16, context, paired)
         if emb_all is None:  # (else: precomputed time_bias(self.unet, t), one row per distinct timestep)
             emb_all = self.time_bias(net, t, x.b)  # the pair repeats the timesteps: row b uses t[b % B]
         state = {"mode": "plain" if uc else "read", "attn_i": 0}
@@ -623,7 +628,7 @@ class DenoiseEngine:
             if taps is not None:
                 taps.append(x)
         hn = ops.groupnorm(x.data, *net.out_gn, batch=x.b, hw=x.hw, eps=1e-5, silu=True)
-        y = self._conv3(Act(hn, x.b, x.h, x.w), net.out_w, net.out_b, cout=self.cfg.out_channels)
+        y = conv3x3(Act(hn, x.b, x.h, x.w), net.out_w, net.out_b, cout=self.cfg.out_channels)
         eps = ops.nhwc_f16_to_nchw_f32(y.data, batch=x.b, c=self.cfg.out_channels, h=x.h, w=x.w)
         if cfg_pair:
             return eps[:b], eps[b:]

@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from . import ops
-from .engine import DenoiseEngine
+from .engine import DenoiseEngine, tensor_key
 
 
 def linear_beta_schedule(n_timestep=1000, linear_start=0.00085, linear_end=0.0120):
@@ -71,19 +71,12 @@ class DenoisePipeline:
         self.t_dev = torch.from_numpy(self.timesteps.astype(np.int64)).to(self.device)
 
     # ---- per-sequence / per-frame preparation --------------------------------------------------
-    @staticmethod
-    def _ident(t):
-        """identity of a tensor's contents as far as the host can tell without a device sync: storage address, view
-        geometry and the in-place version counter (cache entries also hold a strong reference to the tensor, so the
-        address cannot be recycled while the entry lives)"""
-        return (t.untyped_storage().data_ptr(), t.storage_offset(), tuple(t.shape), tuple(t.stride()), t._version)
-
     def reference_bank(self, ref_latent, context, index, first_only=False):
         """Bank K/V for ddim index `index` (appearance 'write' pass + projection), cached per
         (reference tensor, CONTEXT tensor, index): the appearance net runs with the prompt's context
         (cldm.py:1110), so a new prompt with the same reference image needs a new bank.
         first_only: all rows of ref_latent AND of context are the same; compute row 0 and broadcast."""
-        seq = (self._ident(ref_latent), self._ident(context), bool(first_only))
+        seq = (tensor_key(ref_latent), tensor_key(context), bool(first_only))
         if getattr(self, "_bank_seq", None) != seq:
             self._bank_cache.clear()  # a new reference image or prompt: drop the previous sequence's banks (2.3 GB)
             self._bank_seq = seq
@@ -93,8 +86,7 @@ class DenoisePipeline:
             src = ref_latent[:1].contiguous() if first_only else ref_latent
             rb = src.shape[0]
             t = self.t_dev[index].expand(rb).contiguous()
-            bank = self.engine.appearance_write(src, t, context[:rb])
-            hit = self.engine.project_bank(bank, rb)
+            hit = self.engine.bank_kv(src, t, context[:rb])
             self._bank_cache[int(index)] = hit
         return hit
 
@@ -155,8 +147,7 @@ def build_bank_slots(eng: DenoiseEngine, ref_latent, t_vec, context, layout, tok
     per timestep (parallel.BankLayout with ref_batches=1): out_slots [len(t_vec), layout.numel]."""
     tb = t_vec.shape[0]
     ref = ref_latent[:1].expand(tb, -1, -1, -1).contiguous()
-    bank = eng.appearance_write(ref, t_vec, context[:1])
-    kv = eng.project_bank(bank, tb)
+    kv = eng.bank_kv(ref, t_vec, context[:1])
     for (k, vt, n, _), (rows, c), off in zip(kv, layout.layer_shapes, layout.offsets):
         # K [tb*n, c] -> slot j rows; V^T [c, tb*n] -> slot j [c, n]
         out_slots[:, off:off + n * c].view(tb, n, c).copy_(k.view(tb, n, c))

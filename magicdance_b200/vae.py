@@ -6,8 +6,9 @@ ldm/modules/diffusionmodules/model.py:619-652) is the step right after the denoi
 conv3x3, model.py:129-149), three nearest-x2 upsample convs, and ONE single-head attention over all 512 channels in
 the middle block (model.py:179-203) — so it maps onto the kernels the denoiser already has:
 
-  conv3x3            engine.DenoiseEngine._conv3: wgmma implicit GEMM at every level — a 128-pixel TMA box is whole
-                     rows at the 64- and 128-pixel levels and a segment of ONE row (x0 = m0 mod w) at 256 and 512
+  conv3x3            engine.conv3x3: wgmma implicit GEMM at every level — a 128-pixel TMA box is whole rows at the
+                     64- and 128-pixel levels and a segment of ONE row (x0 = m0 mod w) at 256 and 512; the direct
+                     conv for the 3-, 4- and 8-channel ends (conv_in, conv_out, post_quant_conv, quant_conv)
   GroupNorm + swish  ops.groupnorm(eps=1e-6, silu=True) — 4, 8 and 16 channels per group
   1x1 convs          ops.gemm (nin_shortcut, q, k, proj_out); v is produced transposed by swapping operands
   attention (d=512)  ops.gemm (q k^T, scale folded into the q weights) -> ops.softmax_rows -> ops.gemm (P V);
@@ -23,7 +24,7 @@ from __future__ import annotations
 import torch
 
 from . import ops
-from .engine import Act, DenoiseEngine, _f16, _f32, pack_conv1x1, pack_conv3x3
+from .engine import Act, _f16, _f32, conv3x3, pack_conv1x1, pack_conv3x3
 
 PREFIX = "first_stage_model."
 CH_MULT = (1, 2, 4, 4)       # yaml:84-88
@@ -31,7 +32,23 @@ NUM_RES_BLOCKS = 2           # yaml:89
 SCALE_FACTOR = 0.18215       # yaml:9
 GN_EPS = 1e-6                # model.py:45-46
 
-_conv3 = DenoiseEngine._conv3  # the conv dispatcher does not use `self`
+
+def _taker(state_dict, consumed):
+    """take(name): first_stage_model.<name> of the state dict in fp32, its key appended to `consumed`"""
+    def take(name):
+        key = PREFIX + name
+        consumed.append(key)
+        return state_dict[key].detach().float()
+    return take
+
+
+def _center_tap(w1x1, input_scale=1.0):
+    """[O, I, 1, 1] -> a 3x3 kernel whose only non-zero tap is the centre (a 1x1 conv on the direct-conv kernel),
+    applied to its input divided by input_scale"""
+    o, i = w1x1.shape[:2]
+    w3 = torch.zeros(o, i, 3, 3)
+    w3[:, :, 1, 1] = w1x1[:, :, 0, 0] / input_scale
+    return w3
 
 
 class _Res:
@@ -50,6 +67,48 @@ class _Res:
             self.nin_b = _f32(take(name + ".nin_shortcut.bias"), device)
 
 
+def _pack_mid_attention(p, take, a, c, device):
+    """the middle block's single-head attention over all c channels (model.py:152-203) as p.at_gn, p.wq, p.bq, p.wk,
+    p.bk, p.wv, p.wp, p.bp: scale folded into q, v bias into proj_out"""
+    p.at_gn = (_f32(take(a + ".norm.weight"), device), _f32(take(a + ".norm.bias"), device))
+    s = float(c) ** -0.5                                                        # model.py:190
+    p.wq = _f16(take(a + ".q.weight").reshape(c, c) * s, device)
+    p.bq = _f32(take(a + ".q.bias") * s, device)
+    p.wk, p.bk = pack_conv1x1(take(a + ".k.weight"), device), _f32(take(a + ".k.bias"), device)
+    p.wv = pack_conv1x1(take(a + ".v.weight"), device)
+    bv = take(a + ".v.bias")
+    wp = take(a + ".proj_out.weight").reshape(c, c)
+    p.wp = _f16(wp, device)
+    # softmax rows sum to one: P (V + 1 bv^T) = P V + bv^T, and proj_out(o + bv) = proj_out(o) + Wp bv
+    p.bp = _f32(take(a + ".proj_out.bias") + wp @ bv, device)
+
+
+def _res_block(r: _Res, x: Act) -> Act:
+    """ResnetBlock (model.py:129-149)"""
+    h = ops.groupnorm(x.data, *r.gn1, batch=x.b, hw=x.hw, eps=GN_EPS, silu=True)
+    h = conv3x3(Act(h, x.b, x.h, x.w), r.w1, r.b1, cout=r.cout)
+    h2 = ops.groupnorm(h.data, *r.gn2, batch=x.b, hw=x.hw, eps=GN_EPS, silu=True)
+    res = x.data if r.nin_w is None else ops.gemm(x.data, r.nin_w, bias=r.nin_b)
+    return conv3x3(Act(h2, x.b, x.h, x.w), r.w2, r.b2, cout=r.cout, residual=res)
+
+
+def _mid_attention(p, x: Act) -> Act:
+    """AttnBlock (model.py:152-203) of the middle block, weights as _pack_mid_attention left them on the packer p"""
+    n = x.hw
+    assert n % 64 == 0, "the P V product runs as a GEMM over the token axis: h*w must be a multiple of 64"
+    h = ops.groupnorm(x.data, *p.at_gn, batch=x.b, hw=n, eps=GN_EPS, silu=False)
+    q = ops.gemm(h, p.wq, bias=p.bq)                       # already scaled by c^-0.5
+    k = ops.gemm(h, p.wk, bias=p.bk)
+    o = torch.empty_like(q)
+    for b in range(x.b):                                   # one [n, n] score matrix at a time
+        rows = slice(b * n, (b + 1) * n)
+        vt = ops.gemm(p.wv, h[rows])                       # [c, n] == V^T (bias folded into proj_out)
+        s = ops.gemm(q[rows], k[rows])                     # [n, n] = q k^T
+        ops.softmax_rows(s)
+        ops.gemm(s, vt, out=o[rows])                       # [n, c] = P V
+    return Act(ops.gemm(o, p.wp, bias=p.bp, residual=x.data), x.b, x.h, x.w)
+
+
 class PackedVaeDecoder:
     """fp16 repack of `first_stage_model.{post_quant_conv, decoder.*}` (PyTorch-native layouts in, kernel layouts
     out).  `consumed` lists the state-dict keys read, so a test can check nothing is silently ignored."""
@@ -60,36 +119,16 @@ class PackedVaeDecoder:
         self.device = torch.device(device)
         self.consumed = []
         dev = self.device
-
-        def take(name):
-            key = PREFIX + name
-            self.consumed.append(key)
-            return state_dict[key].detach().float()
-
-        # post_quant_conv (autoencoder.py:34,89) on z / scale_factor (ddpm.py:2107): centre tap of a 3x3
-        wpq = take("post_quant_conv.weight")[:, :, 0, 0] / float(scale_factor)      # [4, 4]
-        w3 = torch.zeros(4, 4, 3, 3)
-        w3[:, :, 1, 1] = wpq
-        self.pq_w, self.pq_b = pack_conv3x3(w3, dev), _f32(take("post_quant_conv.bias"), dev)
+        take = _taker(state_dict, self.consumed)
+        # post_quant_conv (autoencoder.py:34,89) on z / scale_factor (ddpm.py:2107)
+        self.pq_w = pack_conv3x3(_center_tap(take("post_quant_conv.weight"), float(scale_factor)), dev)
+        self.pq_b = _f32(take("post_quant_conv.bias"), dev)
         self.in_w = pack_conv3x3(take("decoder.conv_in.weight"), dev)               # [512, 36]
         self.in_b = _f32(take("decoder.conv_in.bias"), dev)
         self.c_mid = self.in_w.shape[0]
         self.mid1 = _Res(take, "decoder.mid.block_1", dev)
         self.mid2 = _Res(take, "decoder.mid.block_2", dev)
-        # middle attention (model.py:152-203)
-        a = "decoder.mid.attn_1"
-        c = self.c_mid
-        self.at_gn = (_f32(take(a + ".norm.weight"), dev), _f32(take(a + ".norm.bias"), dev))
-        s = float(c) ** -0.5                                                        # model.py:190, folded into q
-        self.wq = _f16(take(a + ".q.weight").reshape(c, c) * s, dev)
-        self.bq = _f32(take(a + ".q.bias") * s, dev)
-        self.wk, self.bk = pack_conv1x1(take(a + ".k.weight"), dev), _f32(take(a + ".k.bias"), dev)
-        self.wv = pack_conv1x1(take(a + ".v.weight"), dev)
-        bv = take(a + ".v.bias")
-        wp = take(a + ".proj_out.weight").reshape(c, c)
-        self.wp = _f16(wp, dev)
-        # softmax rows sum to one: P (V + 1 bv^T) = P V + bv^T, and proj_out(o + bv) = proj_out(o) + Wp bv
-        self.bp = _f32(take(a + ".proj_out.bias") + wp @ bv, dev)
+        _pack_mid_attention(self, take, "decoder.mid.attn_1", self.c_mid, dev)
         # up path, executed from the deepest level (model.py:635-643)
         self.up = {}
         for lvl in reversed(range(len(CH_MULT))):
@@ -112,30 +151,6 @@ class VaeDecoder:
         ops.ensure_device()
         self.p = packed
 
-    # ---- blocks ---------------------------------------------------------------------------------
-    def _res(self, r: _Res, x: Act) -> Act:
-        h = ops.groupnorm(x.data, *r.gn1, batch=x.b, hw=x.hw, eps=GN_EPS, silu=True)
-        h = _conv3(None, Act(h, x.b, x.h, x.w), r.w1, r.b1, cout=r.cout)
-        h2 = ops.groupnorm(h.data, *r.gn2, batch=x.b, hw=x.hw, eps=GN_EPS, silu=True)
-        res = x.data if r.nin_w is None else ops.gemm(x.data, r.nin_w, bias=r.nin_b)
-        return _conv3(None, Act(h2, x.b, x.h, x.w), r.w2, r.b2, cout=r.cout, residual=res)
-
-    def _attn(self, x: Act) -> Act:
-        p, n, c = self.p, x.hw, x.c
-        assert n % 64 == 0, "the P V product runs as a GEMM over the token axis: h*w must be a multiple of 64"
-        h = ops.groupnorm(x.data, *p.at_gn, batch=x.b, hw=n, eps=GN_EPS, silu=False)
-        q = ops.gemm(h, p.wq, bias=p.bq)                       # already scaled by c^-0.5
-        k = ops.gemm(h, p.wk, bias=p.bk)
-        o = torch.empty_like(q)
-        for b in range(x.b):                                   # one [n, n] score matrix at a time
-            rows = slice(b * n, (b + 1) * n)
-            vt = ops.gemm(p.wv, h[rows])                       # [c, n] == V^T (bias folded into proj_out)
-            s = ops.gemm(q[rows], k[rows])                     # [n, n] = q k^T
-            ops.softmax_rows(s)
-            ops.gemm(s, vt, out=o[rows])                       # [n, c] = P V
-        return Act(ops.gemm(o, p.wp, bias=p.bp, residual=x.data), x.b, x.h, x.w)
-
-    # ---- the decoder ------------------------------------------------------------------------------
     @torch.no_grad()
     def decode(self, z: torch.Tensor) -> torch.Tensor:
         if not z.is_cuda:
@@ -147,22 +162,21 @@ class VaeDecoder:
         assert z.dim() == 4 and z.shape[1] == 4, "latent must be [B, 4, h, w]"
         b, _, hh, ww = z.shape
         x = ops.nchw_f32_to_nhwc_f16(z.float())                                         # [b*h*w, 4]
-        x = ops.conv3x3_direct(x, p.pq_w, p.pq_b, batch=b, h=hh, w=ww, cin=4, cout=4)    # post_quant_conv(z / scale)
-        x = ops.conv3x3_direct(x, p.in_w, p.in_b, batch=b, h=hh, w=ww, cin=4, cout=p.c_mid)
-        a = Act(x, b, hh, ww)
-        a = self._res(p.mid1, a)
-        a = self._attn(a)
-        a = self._res(p.mid2, a)
+        a = conv3x3(Act(x, b, hh, ww), p.pq_w, p.pq_b, cout=4)                           # post_quant_conv(z / scale)
+        a = conv3x3(a, p.in_w, p.in_b, cout=p.c_mid)
+        a = _res_block(p.mid1, a)
+        a = _mid_attention(p, a)
+        a = _res_block(p.mid2, a)
         for lvl in reversed(range(len(CH_MULT))):
             blocks, ups = p.up[lvl]
             for r in blocks:
-                a = self._res(r, a)
+                a = _res_block(r, a)
             if ups is not None:
                 u = ops.upsample2x(a.data, batch=a.b, h=a.h, w=a.w, c=a.c)               # nearest (model.py:62)
-                a = _conv3(None, Act(u, a.b, 2 * a.h, 2 * a.w), ups[0], ups[1], cout=a.c)
+                a = conv3x3(Act(u, a.b, 2 * a.h, 2 * a.w), ups[0], ups[1], cout=a.c)
         h = ops.groupnorm(a.data, *p.out_gn, batch=a.b, hw=a.hw, eps=GN_EPS, silu=True)
-        y = ops.conv3x3_direct(h, p.out_w, p.out_b, batch=a.b, h=a.h, w=a.w, cin=a.c, cout=p.c_out)
-        return ops.nhwc_f16_to_nchw_f32(y, batch=a.b, c=p.c_out, h=a.h, w=a.w)
+        y = conv3x3(Act(h, a.b, a.h, a.w), p.out_w, p.out_b, cout=p.c_out)
+        return ops.nhwc_f16_to_nchw_f32(y.data, batch=a.b, c=p.c_out, h=a.h, w=a.w)
 
 
 # =====================================================================================================================
@@ -170,30 +184,6 @@ class VaeDecoder:
 # encoded once per sequence (1116.7 GFLOP at 512x512).  Same kernels as the decoder plus ops.im2col3x3(pad="br") for the
 # Downsample's bottom/right padding.
 # =====================================================================================================================
-def _center_tap(w1x1, scale=1.0):
-    """[O, I, 1, 1] -> a 3x3 kernel whose only non-zero tap is the centre (a 1x1 conv on the direct-conv kernel)"""
-    o, i = w1x1.shape[:2]
-    w3 = torch.zeros(o, i, 3, 3)
-    w3[:, :, 1, 1] = w1x1[:, :, 0, 0] * scale
-    return w3
-
-
-class _Attn:
-    """single-head attention over all channels (model.py:152-203): scale folded into q, v bias into proj_out"""
-
-    def __init__(self, take, a, c, device):
-        self.gn = (_f32(take(a + ".norm.weight"), device), _f32(take(a + ".norm.bias"), device))
-        s = float(c) ** -0.5
-        self.wq = _f16(take(a + ".q.weight").reshape(c, c) * s, device)
-        self.bq = _f32(take(a + ".q.bias") * s, device)
-        self.wk, self.bk = pack_conv1x1(take(a + ".k.weight"), device), _f32(take(a + ".k.bias"), device)
-        self.wv = pack_conv1x1(take(a + ".v.weight"), device)
-        bv = take(a + ".v.bias")
-        wp = take(a + ".proj_out.weight").reshape(c, c)
-        self.wp = _f16(wp, device)
-        self.bp = _f32(take(a + ".proj_out.bias") + wp @ bv, device)
-
-
 class PackedVaeEncoder:
     """fp16 repack of `first_stage_model.{encoder.*, quant_conv}`; `consumed` lists the keys read."""
 
@@ -201,12 +191,7 @@ class PackedVaeEncoder:
         self.device = torch.device(device)
         self.consumed = []
         dev = self.device
-
-        def take(name):
-            key = PREFIX + name
-            self.consumed.append(key)
-            return state_dict[key].detach().float()
-
+        take = _taker(state_dict, self.consumed)
         self.in_w = pack_conv3x3(take("encoder.conv_in.weight"), dev)                # [128, 27]
         self.in_b = _f32(take("encoder.conv_in.bias"), dev)
         self.c0 = self.in_w.shape[0]
@@ -220,7 +205,7 @@ class PackedVaeEncoder:
             self.down.append((blocks, ds))
         self.mid1 = _Res(take, "encoder.mid.block_1", dev)
         self.c_mid = self.mid1.cout
-        self.attn = _Attn(take, "encoder.mid.attn_1", self.c_mid, dev)
+        _pack_mid_attention(self, take, "encoder.mid.attn_1", self.c_mid, dev)
         self.mid2 = _Res(take, "encoder.mid.block_2", dev)
         self.out_gn = (_f32(take("encoder.norm_out.weight"), dev), _f32(take("encoder.norm_out.bias"), dev))
         self.out_w = pack_conv3x3(take("encoder.conv_out.weight"), dev)              # [8, 9*512]
@@ -238,23 +223,6 @@ class VaeEncoder:
         ops.ensure_device()
         self.p = packed
 
-    _res = VaeDecoder._res
-
-    def _attn(self, x: Act) -> Act:
-        a, n = self.p.attn, x.hw
-        assert n % 64 == 0, "the P V product runs as a GEMM over the token axis: h*w must be a multiple of 64"
-        h = ops.groupnorm(x.data, *a.gn, batch=x.b, hw=n, eps=GN_EPS, silu=False)
-        q = ops.gemm(h, a.wq, bias=a.bq)
-        k = ops.gemm(h, a.wk, bias=a.bk)
-        o = torch.empty_like(q)
-        for b in range(x.b):
-            rows = slice(b * n, (b + 1) * n)
-            vt = ops.gemm(a.wv, h[rows])
-            s = ops.gemm(q[rows], k[rows])
-            ops.softmax_rows(s)
-            ops.gemm(s, vt, out=o[rows])
-        return Act(ops.gemm(o, a.wp, bias=a.bp, residual=x.data), x.b, x.h, x.w)
-
     @torch.no_grad()
     def encode(self, x: torch.Tensor) -> torch.Tensor:
         if not x.is_cuda:
@@ -266,21 +234,20 @@ class VaeEncoder:
         assert x.dim() == 4 and x.shape[1] == 3 and x.shape[2] % 8 == 0 and x.shape[3] % 8 == 0, "image must be [B, 3, 8h, 8w]"
         b, _, hh, ww = x.shape
         t = ops.nchw_f32_to_nhwc_f16(x.float())                                         # [b*H*W, 3]
-        t = ops.conv3x3_direct(t, p.in_w, p.in_b, batch=b, h=hh, w=ww, cin=3, cout=p.c0)
-        a = Act(t, b, hh, ww)
+        a = conv3x3(Act(t, b, hh, ww), p.in_w, p.in_b, cout=p.c0)
         for blocks, ds in p.down:
             for r in blocks:
-                a = self._res(r, a)
+                a = _res_block(r, a)
             if ds is not None:  # F.pad(x, (0,1,0,1)) + conv(k=3, s=2, p=0)  (model.py:82-84)
                 col = ops.im2col3x3(a.data, batch=a.b, h=a.h, w=a.w, c=a.c, stride=2, pad="br")
                 a = Act(ops.gemm(col, ds[0], bias=ds[1]), a.b, a.h // 2, a.w // 2)
-        a = self._res(p.mid1, a)
-        a = self._attn(a)
-        a = self._res(p.mid2, a)
+        a = _res_block(p.mid1, a)
+        a = _mid_attention(p, a)
+        a = _res_block(p.mid2, a)
         h = ops.groupnorm(a.data, *p.out_gn, batch=a.b, hw=a.hw, eps=GN_EPS, silu=True)
-        y = ops.conv3x3_direct(h, p.out_w, p.out_b, batch=a.b, h=a.h, w=a.w, cin=a.c, cout=p.c_out)
-        y = ops.conv3x3_direct(y, p.q_w, p.q_b, batch=a.b, h=a.h, w=a.w, cin=p.c_out, cout=p.c_out)   # quant_conv
-        return ops.nhwc_f16_to_nchw_f32(y, batch=a.b, c=p.c_out, h=a.h, w=a.w)
+        y = conv3x3(Act(h, a.b, a.h, a.w), p.out_w, p.out_b, cout=p.c_out)
+        y = conv3x3(y, p.q_w, p.q_b, cout=p.c_out)                                         # quant_conv
+        return ops.nhwc_f16_to_nchw_f32(y.data, batch=a.b, c=p.c_out, h=a.h, w=a.w)
 
 
 def posterior_sample(moments: torch.Tensor, noise: torch.Tensor | None = None) -> torch.Tensor:
