@@ -42,7 +42,8 @@ int mdb_device_check(void);
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 int64_t mdb_launch_count(void);
 /* sizeof(mdb_gemm_desc) (which = 0) / sizeof(mdb_attn_desc) (which = 1) / sizeof(mdb_attn_bwd_desc) (which = 2) /
- * sizeof(mdb_gemm_bwd_desc) (which = 3): a binding checks its struct mirrors */
+ * sizeof(mdb_gemm_bwd_desc) (which = 3) / sizeof(mdb_groupnorm_bwd_desc) (which = 4) /
+ * sizeof(mdb_layernorm_bwd_desc) (which = 5): a binding checks its struct mirrors */
 int64_t mdb_abi_struct_bytes(int32_t which);
 
 /* Launch heuristics, process-wide (defaults in parentheses); tests use the setter to force a kernel variant onto small
@@ -225,6 +226,70 @@ int64_t mdb_groupnorm_ws_floats(int32_t c, int32_t batch, int32_t hw);
  * BasicTransformerBlock (attention.py:270-272). */
 int mdb_layernorm_f16(const void* x, const float* gamma, const float* beta, void* y, int64_t rows, int32_t c,
                       float eps, mdb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Backward of mdb_groupnorm_f16: the differentiation of GroupNorm32 (+ SiLU) (util.py:252-254, openaimodel.py:222-226,
+ * 246-248) and Normalize (attention.py:89-90).  Per (batch element b, group g) with n = (c/32) hw, xhat = (x-mean) rstd,
+ * z = gamma xhat + beta, dz = dy silu'(z) (dy without SiLU), A_bc = sum_pix dz, B_bc = sum_pix dz xhat:
+ *   dx = rstd (gamma_c dz - (sum_{c in g} gamma_c A_bc + xhat sum_{c in g} gamma_c B_bc) / n),
+ *   dbeta_c = sum_b A_bc, dgamma_c = sum_b B_bc (batch order).
+ * The statistics are recomputed by the forward's statistics kernel.  Deterministic: fixed-order reductions through
+ * fp32 partial slabs, no atomics on data.  c = c1 + c2 with c1, c2 multiples of 8, c % 32 == 0, 320 <= c <= 2560
+ * (groups of 10 channels or more; the first-stage VAE's 4-channel groups are rejected), batch <= 1024.
+ *   x1, x2, gamma, beta, batch, hw, eps, silu : the forward's arguments (x2 NULL => c2 = 0)
+ *   dy           : fp16 [B][hw][c1+c2], the gradient of the forward's y
+ *   dx1 / dx2    : [B][hw][c1] / [B][hw][c2], MDB_DTYPE_F16 | MDB_DTYPE_F32; NULL = not wanted
+ *   dgamma/dbeta : fp32 [c]; NULL = not wanted (the frozen UNet needs dx only)
+ *   *_accumulate : != 0 adds the gradient to the destination's contents instead of overwriting them
+ *   ws           : fp32 workspace of mdb_groupnorm_bwd_ws_floats(desc) floats, ZERO when first used (the statistics
+ *                  kernel's self-resetting tickets); calls of any shape on one stream may share it
+ * Every pointer but gamma / beta / dgamma / dbeta is 16-byte aligned.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct mdb_groupnorm_bwd_desc {
+  const void* x1; const void* x2; int32_t c1; int32_t c2;
+  const float* gamma; const float* beta;
+  const void* dy;
+  int32_t batch; int32_t hw; float eps; int32_t silu;
+  void* dx1; int32_t dx1_dtype; int32_t dx1_accumulate;
+  void* dx2; int32_t dx2_dtype; int32_t dx2_accumulate;
+  float* dgamma; float* dbeta; int32_t dgamma_accumulate; int32_t dbeta_accumulate;
+  float* ws;
+} mdb_groupnorm_bwd_desc;
+
+int mdb_groupnorm_bwd_f16(const mdb_groupnorm_bwd_desc* desc, mdb_stream_t stream);
+/* workspace floats mdb_groupnorm_bwd_f16 needs for this descriptor; negative MDB_ERR_* for a descriptor it rejects */
+int64_t mdb_groupnorm_bwd_ws_floats(const mdb_groupnorm_bwd_desc* desc);
+
+/* Backward of mdb_layernorm_f16 (nn.LayerNorm norm1/2/3 of BasicTransformerBlock, attention.py:270-272; c = 320, 640,
+ * 1280): with xhat = (x - mean) rstd and dxhat = dy gamma,
+ *   dx = rstd (dxhat - mean(dxhat) - xhat mean(dxhat xhat)),  dgamma = sum_rows dy xhat,  dbeta = sum_rows dy.
+ * One warp per row; mean and rstd are recomputed by the forward's own code (bit-identical statistics).  dgamma / dbeta
+ * are deterministic column sums (per-CTA partials summed in a fixed order).
+ *   x, gamma, rows, c, eps : the forward's arguments; dy fp16 [rows][c]
+ *   dx     : [rows][c], dx_dtype MDB_DTYPE_F16 | MDB_DTYPE_F32; NULL = not wanted
+ *   dgamma / dbeta : fp32 [c]; NULL = not wanted; *_accumulate as above
+ *   ws     : fp32 workspace of mdb_layernorm_bwd_ws_floats(desc) floats (no initial value needed)
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct mdb_layernorm_bwd_desc {
+  const void* x; const float* gamma; const void* dy;
+  int64_t rows; int32_t c; float eps;
+  void* dx; int32_t dx_dtype; int32_t dx_accumulate;
+  float* dgamma; float* dbeta; int32_t dgamma_accumulate; int32_t dbeta_accumulate;
+  float* ws;
+} mdb_layernorm_bwd_desc;
+
+int mdb_layernorm_bwd_f16(const mdb_layernorm_bwd_desc* desc, mdb_stream_t stream);
+int64_t mdb_layernorm_bwd_ws_floats(const mdb_layernorm_bwd_desc* desc);
+
+/* GEGLU activation in the projection's own row order (attention.py:53-56): h = proj(x) is fp16 [m][2n] (row stride
+ * ldh), values in columns [0, n), gates in [n, 2n) — a plain mdb_gemm_f16 with proj.weight / proj.bias as they are.
+ *   forward : out[m][n] = v * gelu_erf(g)                                  (row stride ldo)
+ *   backward: dh[m][2n] = [dout * gelu_erf(g) | dout * v * gelu_erf'(g)]    (row strides lddout, lddh)
+ * n % 8 == 0, row strides multiples of 8, 16-byte aligned pointers.  The interleaved MDB_EPI_GEGLU epilogue is the
+ * inference path; training differentiates this pair and the plain GEMM. */
+int mdb_geglu_f16(const void* h, int64_t ldh, void* out, int64_t ldo, int64_t m, int32_t n, mdb_stream_t stream);
+int mdb_geglu_bwd_f16(const void* h, int64_t ldh, const void* dout, int64_t lddout, void* dh, int64_t lddh, int64_t m,
+                      int32_t n, mdb_stream_t stream);
 
 /* Generic direct 3x3 conv (pad 1, stride 1|2) for shapes the tensor-core path does not take
  * (cin or cout not a multiple of 64): the ControlNet hint encoder (cldm.py:599-615), the 4->320

@@ -63,6 +63,29 @@ class GemmBwdDesc(C.Structure):
     ]
 
 
+class GroupNormBwdDesc(C.Structure):
+    _fields_ = [
+        ("x1", c_void_p), ("x2", c_void_p), ("c1", c_int32), ("c2", c_int32),
+        ("gamma", c_void_p), ("beta", c_void_p),
+        ("dy", c_void_p),
+        ("batch", c_int32), ("hw", c_int32), ("eps", c_float), ("silu", c_int32),
+        ("dx1", c_void_p), ("dx1_dtype", c_int32), ("dx1_accumulate", c_int32),
+        ("dx2", c_void_p), ("dx2_dtype", c_int32), ("dx2_accumulate", c_int32),
+        ("dgamma", c_void_p), ("dbeta", c_void_p), ("dgamma_accumulate", c_int32), ("dbeta_accumulate", c_int32),
+        ("ws", c_void_p),
+    ]
+
+
+class LayerNormBwdDesc(C.Structure):
+    _fields_ = [
+        ("x", c_void_p), ("gamma", c_void_p), ("dy", c_void_p),
+        ("rows", c_int64), ("c", c_int32), ("eps", c_float),
+        ("dx", c_void_p), ("dx_dtype", c_int32), ("dx_accumulate", c_int32),
+        ("dgamma", c_void_p), ("dbeta", c_void_p), ("dgamma_accumulate", c_int32), ("dbeta_accumulate", c_int32),
+        ("ws", c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/magicdance_b200.h declares
 SIGNATURES = {
     "mdb_abi_version": (c_int32, []),
@@ -83,6 +106,13 @@ SIGNATURES = {
                                     c_int32, c_int32, c_float, c_int32, c_int32, c_void_p]),
     "mdb_groupnorm_ws_floats": (c_int64, [c_int32, c_int32, c_int32]),
     "mdb_layernorm_f16": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_float, c_void_p]),
+    "mdb_groupnorm_bwd_f16": (c_int32, [C.POINTER(GroupNormBwdDesc), c_void_p]),
+    "mdb_groupnorm_bwd_ws_floats": (c_int64, [C.POINTER(GroupNormBwdDesc)]),
+    "mdb_layernorm_bwd_f16": (c_int32, [C.POINTER(LayerNormBwdDesc), c_void_p]),
+    "mdb_layernorm_bwd_ws_floats": (c_int64, [C.POINTER(LayerNormBwdDesc)]),
+    "mdb_geglu_f16": (c_int32, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int32, c_void_p]),
+    "mdb_geglu_bwd_f16": (c_int32, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int32,
+                                    c_void_p]),
     "mdb_conv3x3_direct_f16": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
                                          c_int32, c_int32, c_int32, c_int32, c_void_p]),
     "mdb_im2col3x3_f16": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p]),
@@ -131,7 +161,8 @@ def load():
     if lib.mdb_abi_version() != ABI_VERSION:
         raise RuntimeError(f"magicdance_b200: ABI version mismatch ({lib.mdb_abi_version()} != {ABI_VERSION}); "
                            "rebuild the library")
-    for which, mirror in ((0, GemmDesc), (1, AttnDesc), (2, AttnBwdDesc), (3, GemmBwdDesc)):
+    for which, mirror in ((0, GemmDesc), (1, AttnDesc), (2, AttnBwdDesc), (3, GemmBwdDesc), (4, GroupNormBwdDesc),
+                          (5, LayerNormBwdDesc)):
         if lib.mdb_abi_struct_bytes(which) != C.sizeof(mirror):
             raise RuntimeError(f"magicdance_b200: {mirror.__name__} mirrors {C.sizeof(mirror)} bytes, the library's "
                                f"struct has {lib.mdb_abi_struct_bytes(which)}: the binding and the library disagree")

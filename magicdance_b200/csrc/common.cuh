@@ -320,6 +320,56 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + __expf(-x)); }
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
+// derivatives: silu'(x) = s (1 + x (1 - s)) with s = sigmoid(x); gelu'(x) = Phi(x) + x phi(x)
+__device__ __forceinline__ float dsilu(float x) {
+  const float s = 1.0f / (1.0f + __expf(-x));
+  return s * (1.0f + x * (1.0f - s));
+}
+__device__ __forceinline__ float dgelu_erf(float x) {
+  return 0.5f * (1.0f + erff(x * 0.70710678118654752f)) + x * 0.39894228040143268f * __expf(-0.5f * x * x);
+}
+
+// ---- gradient destinations of the backward kernels -------------------------------------------------
+struct GbOut {  // fp16 or fp32 rows, overwritten or accumulated into; p == nullptr: dropped
+  void* p;
+  long long ld;
+  int f32, acc;
+};
+
+__device__ __forceinline__ void gb_store2(const GbOut& o, long long row, int col, float v0, float v1) {
+  if (o.p == nullptr) return;
+  if (o.f32) {
+    float2* d = reinterpret_cast<float2*>(static_cast<float*>(o.p) + row * o.ld + col);
+    if (o.acc) {
+      const float2 x = *d;
+      v0 += x.x;
+      v1 += x.y;
+    }
+    *d = make_float2(v0, v1);
+  } else {
+    __half2* d = reinterpret_cast<__half2*>(static_cast<__half*>(o.p) + row * o.ld + col);
+    if (o.acc) {
+      const float2 x = __half22float2(*d);
+      v0 += x.x;
+      v1 += x.y;
+    }
+    *d = __floats2half2_rn(v0, v1);
+  }
+}
 #endif  // __CUDACC__
+
+inline GbOut gb_out(void* p, long long ld, int dtype, int acc) {
+  GbOut o;
+  o.p = p;
+  o.ld = ld;
+  o.f32 = dtype == MDB_DTYPE_F32;
+  o.acc = acc != 0;
+  return o;
+}
+
+// second pass of a fixed-order column sum (gemm_bwd.cu): out[seg * stride + col] (+)= sum over q < parts, in order, of
+// ws[(seg * parts + q) * n + col], for seg < segs and col < n.  Counts its launch.
+int launch_colsum_finalize(const float* ws, int n, int segs, int parts, float* out, long long stride, int acc,
+                           cudaStream_t st);
 
 }  // namespace mdb

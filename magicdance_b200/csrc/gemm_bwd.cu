@@ -32,12 +32,6 @@ constexpr int kGbStageBytes = kGbABytes + (kGbN / 64) * kGbChunk;
 constexpr int kGbSmem = kGbStages * kGbStageBytes + 1024;  // two CTAs per SM
 constexpr int kBiasRows = 256;  // rows per partial column sum
 
-struct GbOut {  // a gradient destination: fp16 or fp32 rows, overwritten or accumulated into; p == nullptr: dropped
-  void* p;
-  long long ld;
-  int f32, acc;
-};
-
 struct GemmBwdKParams {
   CUtensorMap tmD;   // dD: TA = 0 [128 x 64] boxes (4-D pixel boxes in conv mode); TA = 1 [64 x 64] boxes
   CUtensorMap tmB;   // TA = 0: the forward's B, [64 x 64] boxes; TA = 1: the forward's A (4-D pixel boxes in conv mode)
@@ -53,27 +47,6 @@ struct GemmBwdKParams {
   int w, hw, cs;     // conv pixel geometry: TA = 0 the row tiles (stride 1), TA = 1 the forward's output pixels
   int k1;            // TA = 1 plain: columns taken from tmB, the rest from tmB2
 };
-
-__device__ __forceinline__ void gb_store2(const GbOut& o, long long row, int col, float v0, float v1) {
-  if (o.p == nullptr) return;
-  if (o.f32) {
-    float2* d = reinterpret_cast<float2*>(static_cast<float*>(o.p) + row * o.ld + col);
-    if (o.acc) {
-      const float2 x = *d;
-      v0 += x.x;
-      v1 += x.y;
-    }
-    *d = make_float2(v0, v1);
-  } else {
-    __half2* d = reinterpret_cast<__half2*>(static_cast<__half*>(o.p) + row * o.ld + col);
-    if (o.acc) {
-      const float2 x = __half22float2(*d);
-      v0 += x.x;
-      v1 += x.y;
-    }
-    *d = __floats2half2_rn(v0, v1);
-  }
-}
 
 __device__ __forceinline__ void gb_put(const GemmBwdKParams& p, long long row, int col, float v0, float v1) {
   if (col < p.split_col) gb_store2(p.out[0], row, col, v0, v1);
@@ -415,15 +388,6 @@ static int launch_bwd_gemm(int ta, GemmBwdKParams& kp, int tiles_x, int splits, 
   return MDB_OK;
 }
 
-static GbOut gb_out(void* p, long long ld, int dtype, int acc) {
-  GbOut o;
-  o.p = p;
-  o.ld = ld;
-  o.f32 = dtype == MDB_DTYPE_F32;
-  o.acc = acc != 0;
-  return o;
-}
-
 static int run_da(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st) {
   const mdb_gemm_desc* f = &g->fwd;
   GemmBwdKParams kp;
@@ -515,11 +479,17 @@ static int run_dbias(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t 
   const dim3 grid((f->n + 31) / 32, pl.bias_segs * pl.bias_parts);
   MDB_CHECK_CUDA(launch_pdl(colsum_partial_kernel, grid, dim3(32, 8), 0, st, static_cast<const __half*>(g->dd),
                             (long long)g->lddd, f->m, f->n, pl.bias_rpb, pl.bias_parts, g->ws));
-  const long long total = static_cast<long long>(pl.bias_segs) * f->n;
+  count_launch();
+  return launch_colsum_finalize(g->ws, f->n, pl.bias_segs, pl.bias_parts, g->dbias,
+                                f->bias_batch_stride != 0 ? f->bias_batch_stride : 0, g->dbias_accumulate, st);
+}
+
+int launch_colsum_finalize(const float* ws, int n, int segs, int parts, float* out, long long stride, int acc,
+                           cudaStream_t st) {
+  const long long total = static_cast<long long>(segs) * n;
   MDB_CHECK_CUDA(launch_pdl(colsum_finalize_kernel, dim3(static_cast<unsigned>((total + 255) / 256)), dim3(256), 0, st,
-                            static_cast<const float*>(g->ws), f->n, pl.bias_segs, pl.bias_parts, g->dbias,
-                            (long long)(f->bias_batch_stride != 0 ? f->bias_batch_stride : 0), g->dbias_accumulate));
-  count_launch(2);
+                            ws, n, segs, parts, out, stride, acc));
+  count_launch();
   return MDB_OK;
 }
 

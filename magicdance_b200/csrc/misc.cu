@@ -548,6 +548,10 @@ extern "C" int64_t mdb_abi_struct_bytes(int32_t which) {
       return (int64_t)sizeof(mdb_attn_bwd_desc);
     case 3:
       return (int64_t)sizeof(mdb_gemm_bwd_desc);
+    case 4:
+      return (int64_t)sizeof(mdb_groupnorm_bwd_desc);
+    case 5:
+      return (int64_t)sizeof(mdb_layernorm_bwd_desc);
     default:
       return -1;
   }

@@ -15,24 +15,10 @@
 //   gn_apply_kernel     y = x * a_c + b_c [+ SiLU], 8 channels per thread.
 // The input may be the channel concatenation of two tensors, which is how torch.cat([h, skip], 1) (cldm.py:104)
 // disappears: the normalised copy is the only concatenated buffer.
-#include "common.cuh"
+#include "norm.cuh"
 
 namespace mdb {
 
-__device__ __forceinline__ const uint4* gn_src(const __half* x1, int c1, const __half* x2, int c2, long long row,
-                                                int ch) {
-  // channel ch (multiple of 8) of concatenated row -> address of its 16-byte vector
-  return (ch < c1) ? reinterpret_cast<const uint4*>(x1 + row * c1 + ch)
-                   : reinterpret_cast<const uint4*>(x2 + row * c2 + (ch - c1));
-}
-
-// pivot of group g of batch element b: the group's first channel at pixel 0
-__device__ __forceinline__ float gn_pivot(const __half* x1, int c1, const __half* x2, int c2, int b, int hw, int ch) {
-  return (ch < c1) ? __half2float(x1[static_cast<long long>(b) * hw * c1 + ch])
-                   : __half2float(x2[static_cast<long long>(b) * hw * c2 + (ch - c1)]);
-}
-
-constexpr int kGnMaxBatch = 1024;     // batch elements of the two-kernel path (size of the ticket region)
 constexpr int kGnFinalThreads = 256;  // threads of the last CTA that fold the partials (4 slices x 64 entries)
 
 // ws layout (floats): [kGnMaxBatch] tickets (uint, zero at first use, self-resetting; a FIXED region so that calls
@@ -317,24 +303,8 @@ __global__ void layernorm_kernel(const __half* __restrict__ x, const float* __re
   if (warp >= rows) return;
   const __half2* xr = reinterpret_cast<const __half2*>(x + static_cast<long long>(warp) * c);
   float2 v[VPL];
-  float s = 0.f;
-#pragma unroll
-  for (int i = 0; i < VPL; ++i) {
-    v[i] = __half22float2(xr[lane + i * 32]);
-    s += v[i].x + v[i].y;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const float mean = s / c;
-  float q = 0.f;
-#pragma unroll
-  for (int i = 0; i < VPL; ++i) {
-    const float dx = v[i].x - mean, dy = v[i].y - mean;
-    q += dx * dx + dy * dy;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-  const float rstd = rsqrtf(q / c + eps);
+  float mean, rstd;
+  ln_row_stats<VPL>(xr, lane, c, eps, v, mean, rstd);
   __half2* yr = reinterpret_cast<__half2*>(y + static_cast<long long>(warp) * c);
 #pragma unroll
   for (int i = 0; i < VPL; ++i) {
@@ -345,13 +315,9 @@ __global__ void layernorm_kernel(const __half* __restrict__ x, const float* __re
   }
 }
 
-}  // namespace mdb
-
-using namespace mdb;
-
 // rows per stats CTA / stats grid: ~296 CTAs (2 per SM) in total, whole multiples of the row-phase count,
 // at most 8 rows per thread
-static void gn_stats_geometry(int c, int batch, int hw, int* threads_out, int* rows_per_cta_out, int* nblk_out) {
+void gn_stats_geometry(int c, int batch, int hw, int* threads_out, int* rows_per_cta_out, int* nblk_out) {
   const int vecs = c / 8;
   int threads = ((512 / vecs) * vecs);  // whole number of row phases
   if (threads < vecs) threads = vecs;
@@ -364,6 +330,25 @@ static void gn_stats_geometry(int c, int batch, int hw, int* threads_out, int* r
   *rows_per_cta_out = rows_per_cta;
   *nblk_out = (hw + rows_per_cta - 1) / rows_per_cta;
 }
+
+int launch_gn_stats(const __half* x1, int c1, const __half* x2, int c2, float* ws, int batch, int hw,
+                    cudaStream_t st) {
+  const int c = c1 + c2;
+  int threads, rows_per_cta, nblk;
+  gn_stats_geometry(c, batch, hw, &threads, &rows_per_cta, &nblk);
+  const int rstride = threads / (c / 8);
+  size_t smem_stats = static_cast<size_t>(2) * rstride * c * sizeof(float);
+  if (smem_stats < 256 * sizeof(float)) smem_stats = 256 * sizeof(float);
+  MDB_REQUIRE(threads >= kGnFinalThreads && smem_stats <= 48 * 1024, "mdb_groupnorm_f16: unsupported width %d", c);
+  MDB_REQUIRE(batch <= kGnMaxBatch, "mdb_groupnorm_f16: batch %d > %d", batch, kGnMaxBatch);
+  MDB_CHECK_CUDA(launch_pdl(gn_stats_kernel, dim3(nblk, batch), dim3(threads), smem_stats, st, x1, c1, x2, c2, ws,
+                            batch, hw, rows_per_cta));
+  return MDB_OK;
+}
+
+}  // namespace mdb
+
+using namespace mdb;
 
 // floats of workspace mdb_groupnorm_f16 needs for the two-kernel path (0 when the call takes the single-launch
 // cluster path).  The workspace must be ZERO when first used (tickets); the kernels leave it reusable.
@@ -411,16 +396,9 @@ extern "C" int mdb_groupnorm_f16(const void* x1, int32_t c1, const void* x2, int
   MDB_REQUIRE(c % 32 == 0 && c1 % 8 == 0 && c2 % 8 == 0 && (c / 32 >= 8 || c / 32 == 4),
               "mdb_groupnorm_f16: channels must be multiples of 8, c %% 32 == 0 and c/32 >= 8 or == 4 (c1=%d c2=%d)", c1, c2);
   MDB_REQUIRE(c / 8 <= 512, "mdb_groupnorm_f16: too many channels (%d)", c);
-  int threads, rows_per_cta, nblk;
-  gn_stats_geometry(c, batch, hw, &threads, &rows_per_cta, &nblk);
-  const int rstride = threads / (c / 8);
-  size_t smem_stats = static_cast<size_t>(2) * rstride * c * sizeof(float);
-  if (smem_stats < 256 * sizeof(float)) smem_stats = 256 * sizeof(float);
-  MDB_REQUIRE(threads >= kGnFinalThreads && smem_stats <= 48 * 1024, "mdb_groupnorm_f16: unsupported width %d", c);
-  MDB_REQUIRE(batch <= kGnMaxBatch, "mdb_groupnorm_f16: batch %d > %d", batch, kGnMaxBatch);
-  dim3 grid(nblk, batch);
-  MDB_CHECK_CUDA(launch_pdl(gn_stats_kernel, grid, dim3(threads), smem_stats, st, static_cast<const __half*>(x1), c1,
-                            static_cast<const __half*>(x2), c2, ws, batch, hw, rows_per_cta));
+  const int rc = launch_gn_stats(static_cast<const __half*>(x1), c1, static_cast<const __half*>(x2), c2, ws, batch, hw,
+                                 st);
+  if (rc) return rc;
   {
     // ~2-4 CTAs per SM; each CTA pays a c-element (scale, shift) setup, so rows per CTA grow with c
     int rows_apply = (batch * hw + 443) / 444;

@@ -334,7 +334,9 @@ class TcGemm(torch.autograd.Function):
 def tc_gemm(a, w, *, a_param=None, w_param=None, bias=None, bias_batch_stride=0, rows_per_batch=0, residual=None,
             a2=None, conv=None, conv_stride=1, splits=0, m=None, epilogue=EPI_NONE, ln_u=None):
     """Differentiable gemm() (TcGemm).  GEGLU and the folded LayerNorm have no backward kernel and are refused here,
-    before anything runs."""
+    before anything runs.  Training composes the unfused pieces instead: tc_gemm with proj.weight / proj.bias then
+    geglu(), and layer_norm() then tc_gemm (norm2 -> attn2.to_q) — the fold never materialises the normalised rows
+    that the weight gradient needs."""
     if epilogue != EPI_NONE:
         raise RuntimeError("magicdance_b200.tc_gemm: the GEGLU epilogue has no backward kernel")
     if ln_u is not None:
@@ -484,6 +486,197 @@ def layernorm(x, gamma, beta, eps=1e-5, out=None):
     _lib.check(lib.mdb_layernorm_f16(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), out.data_ptr(), rows, c, eps,
                                      _stream()), "layernorm_f16")
     return out
+
+
+def _dx_out(t, shape, dtype, device, name):
+    """a dx destination of the norm backwards: `t` (contiguous fp16 / fp32) or a new tensor"""
+    t = _grad_out(t, shape, dtype, device, name)
+    assert t.is_contiguous(), name
+    return t
+
+
+def _param_grad(t, n, device, name):
+    """an fp32 [n] gradient destination of gamma / beta: `t` or a new tensor"""
+    if t is None:
+        t = torch.empty(n, dtype=torch.float32, device=device)
+    _chk(t, torch.float32, name)
+    assert t.is_contiguous() and t.numel() == n, (name, t.shape, n)
+    return t
+
+
+def groupnorm_backward(x1, gamma, beta, dy, *, batch, hw, eps, silu, x2=None, grads=("x", "gamma", "beta"),
+                       dx_dtype=torch.float16, out_dx1=None, out_dx2=None, out_dgamma=None, out_dbeta=None,
+                       accumulate=()):
+    """Gradients of y = groupnorm(x1, gamma, beta, batch=, hw=, eps=, silu=, x2=) from dy = dL/dy (fp16
+    [batch*hw, c1+c2]), csrc/norm_bwd.cu; the statistics are recomputed.  `grads` names the gradients to compute among
+    "x" (dx1, and dx2 with x2), "gamma" and "beta".  Each goes to its out_* tensor when given (its dtype is then the
+    gradient's dtype) or to a new one of dx_dtype (dgamma / dbeta: fp32); names in `accumulate` ("x", "x2", "gamma",
+    "beta") add into the out_* tensor instead of overwriting it.  Returns (dx1, dx2, dgamma, dbeta), None for a
+    gradient not requested.  Deterministic.  Groups narrower than 10 channels (the VAE's) are rejected."""
+    lib = _lib.load()
+    _chk(x1, torch.float16, "x1")
+    _chk(dy, torch.float16, "dy")
+    _chk(gamma, torch.float32, "gamma")
+    _chk(beta, torch.float32, "beta")
+    c1 = x1.shape[-1]
+    c2 = 0
+    if x2 is not None:
+        _chk(x2, torch.float16, "x2")
+        c2 = x2.shape[-1]
+        assert x2.is_contiguous()
+    assert x1.is_contiguous() and dy.is_contiguous() and tuple(dy.shape) == (batch * hw, c1 + c2), dy.shape
+    dev = x1.device
+    d = _lib.GroupNormBwdDesc()
+    d.x1, d.x2, d.c1, d.c2 = x1.data_ptr(), _ptr(x2), c1, c2
+    d.gamma, d.beta, d.dy = gamma.data_ptr(), beta.data_ptr(), dy.data_ptr()
+    d.batch, d.hw, d.eps, d.silu = batch, hw, eps, int(silu)
+    acc = set(accumulate)
+    dx1 = dx2 = dgamma = dbeta = None
+    if "x" in grads:
+        dx1 = _dx_out(out_dx1, (batch * hw, c1), dx_dtype, dev, "out_dx1")
+        d.dx1, d.dx1_dtype, d.dx1_accumulate = dx1.data_ptr(), _DTYPES[dx1.dtype], "x" in acc
+        if x2 is not None:
+            dx2 = _dx_out(out_dx2, (batch * hw, c2), dx_dtype, dev, "out_dx2")
+            d.dx2, d.dx2_dtype, d.dx2_accumulate = dx2.data_ptr(), _DTYPES[dx2.dtype], "x2" in acc
+    if "gamma" in grads:
+        dgamma = _param_grad(out_dgamma, c1 + c2, dev, "out_dgamma")
+        d.dgamma, d.dgamma_accumulate = dgamma.data_ptr(), "gamma" in acc
+    if "beta" in grads:
+        dbeta = _param_grad(out_dbeta, c1 + c2, dev, "out_dbeta")
+        d.dbeta, d.dbeta_accumulate = dbeta.data_ptr(), "beta" in acc
+    need = int(lib.mdb_groupnorm_bwd_ws_floats(C.byref(d)))
+    if need < 0:
+        _lib.check(need, "groupnorm_bwd_f16")
+    # the statistics kernel's tickets must be zero at first use (_workspace(zero=True)); the kernels leave them so
+    d.ws = _workspace("gn_bwd", need, torch.float32, dev, zero=True).data_ptr()
+    _lib.check(lib.mdb_groupnorm_bwd_f16(C.byref(d), _stream()), "groupnorm_bwd_f16")
+    return dx1, dx2, dgamma, dbeta
+
+
+def layernorm_backward(x, gamma, dy, *, eps=1e-5, grads=("x", "gamma", "beta"), dx_dtype=torch.float16, out_dx=None,
+                       out_dgamma=None, out_dbeta=None, accumulate=()):
+    """Gradients of y = layernorm(x, gamma, beta, eps) from dy (fp16 [rows, c]), csrc/norm_bwd.cu; mean and rstd are
+    recomputed by the forward's code.  grads / out_* / accumulate as in groupnorm_backward ("x", "gamma", "beta").
+    Returns (dx, dgamma, dbeta).  Deterministic."""
+    lib = _lib.load()
+    _chk(x, torch.float16, "x")
+    _chk(dy, torch.float16, "dy")
+    _chk(gamma, torch.float32, "gamma")
+    assert x.is_contiguous() and dy.is_contiguous() and dy.shape == x.shape, (x.shape, dy.shape)
+    rows, c = x.shape
+    dev = x.device
+    d = _lib.LayerNormBwdDesc()
+    d.x, d.gamma, d.dy, d.rows, d.c, d.eps = x.data_ptr(), gamma.data_ptr(), dy.data_ptr(), rows, c, eps
+    acc = set(accumulate)
+    dx = dgamma = dbeta = None
+    if "x" in grads:
+        dx = _dx_out(out_dx, (rows, c), dx_dtype, dev, "out_dx")
+        d.dx, d.dx_dtype, d.dx_accumulate = dx.data_ptr(), _DTYPES[dx.dtype], "x" in acc
+    if "gamma" in grads:
+        dgamma = _param_grad(out_dgamma, c, dev, "out_dgamma")
+        d.dgamma, d.dgamma_accumulate = dgamma.data_ptr(), "gamma" in acc
+    if "beta" in grads:
+        dbeta = _param_grad(out_dbeta, c, dev, "out_dbeta")
+        d.dbeta, d.dbeta_accumulate = dbeta.data_ptr(), "beta" in acc
+    need = int(lib.mdb_layernorm_bwd_ws_floats(C.byref(d)))
+    if need < 0:
+        _lib.check(need, "layernorm_bwd_f16")
+    d.ws = _workspace("ln_bwd", need, torch.float32, dev).data_ptr()
+    _lib.check(lib.mdb_layernorm_bwd_f16(C.byref(d), _stream()), "layernorm_bwd_f16")
+    return dx, dgamma, dbeta
+
+
+def _geglu_forward(h):
+    lib = _lib.load()
+    _chk(h, torch.float16, "h")
+    assert h.dim() == 2 and h.stride(1) == 1 and h.shape[1] % 2 == 0
+    m, n = h.shape[0], h.shape[1] // 2
+    out = torch.empty((m, n), dtype=torch.float16, device=h.device)
+    _lib.check(lib.mdb_geglu_f16(h.data_ptr(), h.stride(0), out.data_ptr(), out.stride(0), m, n, _stream()), "geglu_f16")
+    return out
+
+
+def geglu_backward(h, dout):
+    """Gradient of out = geglu(h) from dout (fp16 [M, N], row stride a multiple of 8): dh [M, 2N] =
+    [dout * gelu(g) | dout * v * gelu'(g)] in the projection's own row order, ready to be gemm_backward's dd."""
+    lib = _lib.load()
+    _chk(h, torch.float16, "h")
+    _chk(dout, torch.float16, "dout")
+    assert h.dim() == 2 and h.stride(1) == 1 and dout.dim() == 2 and dout.stride(1) == 1
+    m, n = dout.shape
+    assert tuple(h.shape) == (m, 2 * n), (h.shape, dout.shape)
+    dh = torch.empty((m, 2 * n), dtype=torch.float16, device=h.device)
+    _lib.check(lib.mdb_geglu_bwd_f16(h.data_ptr(), h.stride(0), dout.data_ptr(), dout.stride(0), dh.data_ptr(),
+                                     dh.stride(0), m, n, _stream()), "geglu_bwd_f16")
+    return dh
+
+
+class GroupNorm(torch.autograd.Function):
+    """groupnorm() as an autograd op: fp16 gradients to x1 and x2, fp32 ones to gamma and beta (the nn.Parameters
+    themselves, no layout change).  Positional arguments in group_norm()'s order."""
+
+    @staticmethod
+    def forward(ctx, x1, gamma, beta, x2, batch, hw, eps, silu):
+        ctx.save_for_backward(x1, gamma, beta, x2)
+        ctx.kw = dict(batch=batch, hw=hw, eps=eps, silu=silu)
+        return groupnorm(x1, gamma, beta, x2=x2, **ctx.kw)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x1, gamma, beta, x2 = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        grads = [nm for nm, want in (("x", need[0] or need[3]), ("gamma", need[1]), ("beta", need[2])) if want]
+        dx1, dx2, dgamma, dbeta = groupnorm_backward(x1, gamma, beta, dy.contiguous(), x2=x2, grads=grads, **ctx.kw)
+        return dx1, dgamma, dbeta, dx2, None, None, None, None
+
+
+def group_norm(x1, gamma, beta, *, batch, hw, eps, silu, x2=None):
+    """Differentiable groupnorm() (GroupNorm): x1 [batch*hw, c1] (and x2 [batch*hw, c2]) fp16, gamma / beta fp32."""
+    return GroupNorm.apply(x1, gamma, beta, x2, batch, hw, eps, silu)
+
+
+class LayerNorm(torch.autograd.Function):
+    """layernorm() as an autograd op: an fp16 gradient to x, fp32 ones to gamma and beta."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, eps):
+        ctx.save_for_backward(x, gamma)
+        ctx.eps = eps
+        return layernorm(x, gamma, beta, eps)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, gamma = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        grads = [nm for nm, want in (("x", need[0]), ("gamma", need[1]), ("beta", need[2])) if want]
+        dx, dgamma, dbeta = layernorm_backward(x, gamma, dy.contiguous(), eps=ctx.eps, grads=grads)
+        return dx, dgamma, dbeta, None
+
+
+def layer_norm(x, gamma, beta, *, eps=1e-5):
+    """Differentiable layernorm() (LayerNorm): x fp16 [rows, c], gamma / beta fp32."""
+    return LayerNorm.apply(x, gamma, beta, eps)
+
+
+class Geglu(torch.autograd.Function):
+    """The GEGLU activation as an autograd op: out = v * gelu_erf(g) of h = [v | g] (fp16 [M, 2N], the output of a
+    plain tc_gemm with proj.weight / proj.bias as they are), gradient dh in the same order."""
+
+    @staticmethod
+    def forward(ctx, h):
+        ctx.save_for_backward(h)
+        return _geglu_forward(h)
+
+    @staticmethod
+    def backward(ctx, dout):
+        (h,) = ctx.saved_tensors
+        return geglu_backward(h, _rows8(dout))
+
+
+def geglu(h):
+    """GEGLU forward (attention.py:53-56) on h = proj(x) in the parameter's row order: fp16 [M, 2N] -> [M, N]
+    (csrc/norm_bwd.cu); differentiable (Geglu)."""
+    return Geglu.apply(h)
 
 
 def conv3x3_direct(x, wt, bias, *, batch, h, w, cin, cout, stride=1, silu=False, residual=None, out=None):

@@ -63,7 +63,7 @@ def attn_case(b, d, nq, n0, n1=0):
            flops=4.0 * b * 8 * nq * (n0 + n1) * d)
 
 
-def timeit_eager(name, fn, reps=20, flops=None):
+def timeit_eager(name, fn, reps=20, flops=None, bytes_=None):
     """CUDA events around `reps` eager calls (for torch autograd, which a CUDA graph cannot capture here)"""
     for _ in range(3):
         fn()
@@ -78,6 +78,8 @@ def timeit_eager(name, fn, reps=20, flops=None):
         torch.cuda.synchronize()
         best = min(best, e0.elapsed_time(e1) * 1e3 / reps)
     extra = f"  {flops / best / 1e6:8.1f} TFLOP/s" if flops else ""
+    if bytes_:
+        extra += f"  {bytes_ / best / 1e3:8.1f} GB/s"
     print(f"{name:58s} {best:9.2f} us{extra}", flush=True)
 
 
@@ -149,9 +151,61 @@ def gemm_bwd_case(m, n, k, conv=None, stride=1):
                      lambda: torch.autograd.grad(F.linear(at, wt), (at, wt), dd), flops=3 * fl)
 
 
+def norm_bwd_cases():
+    """our GroupNorm(+SiLU) / LayerNorm / GEGLU backward against torch's own backward kernels on the same fp16 tensors
+    (torch.autograd.grad through a recorded forward, so only the backward runs).  Bytes are computed from shapes:
+    GroupNorm reads x in the statistics pass and x + dy in each of its two data passes and writes dx (12 bytes per
+    element); LayerNorm reads x + dy once and writes dx (6); GEGLU reads h and dout and writes dh (10 per output)."""
+    import torch.nn.functional as F
+    b = 4  # BASELINE config 5: 4 samples at latent 64x64
+    for hw, c1, c2 in ((4096, 320, 0), (4096, 320, 320), (4096, 640, 320), (1024, 640, 0), (1024, 1280, 640),
+                       (256, 1280, 0), (256, 1280, 1280), (64, 1280, 1280)):
+        c, e = c1 + c2, b * hw * (c1 + c2)
+        x1, x2 = h(b * hw, c1), (h(b * hw, c2) if c2 else None)
+        g_, b_, dy = f(c), f(c), h(b * hw, c)
+        tag = f"B={b} hw={hw} c={c1}+{c2}"
+        kw = dict(batch=b, hw=hw, eps=1e-5, silu=True, x2=x2)
+        timeit(f"ours  groupnorm+silu bwd dx       {tag}",
+               lambda: ops.groupnorm_backward(x1, g_, b_, dy, grads=("x",), **kw), bytes_=12.0 * e)
+        timeit(f"ours  groupnorm+silu bwd dx,dg,db {tag}",
+               lambda: ops.groupnorm_backward(x1, g_, b_, dy, **kw), bytes_=12.0 * e)
+        xt = (torch.cat([x1, x2], 1) if c2 else x1).view(b, hw, c).permute(0, 2, 1).detach().requires_grad_()
+        gt, bt = g_.half().requires_grad_(), b_.half().requires_grad_()
+        y = F.silu(F.group_norm(xt, 32, gt, bt, 1e-5))
+        dyt = dy.view(b, hw, c).permute(0, 2, 1)
+        timeit_eager(f"torch groupnorm+silu bwd dx,dg,db {tag}",
+                     lambda: torch.autograd.grad(y, (xt, gt, bt), dyt, retain_graph=True))
+    for rows, c in ((16384, 320), (4096, 640), (1024, 1280)):
+        x, g_, dy = h(rows, c), f(c), h(rows, c)
+        timeit(f"ours  layernorm bwd dx       rows={rows} c={c}",
+               lambda: ops.layernorm_backward(x, g_, dy, grads=("x",)), bytes_=6.0 * rows * c)
+        timeit(f"ours  layernorm bwd dx,dg,db rows={rows} c={c}", lambda: ops.layernorm_backward(x, g_, dy),
+               bytes_=6.0 * rows * c)
+        xt, gt, bt = x.clone().requires_grad_(), g_.half().requires_grad_(), f(c).half().requires_grad_()
+        y = F.layer_norm(xt, (c,), gt, bt, 1e-5)
+        timeit_eager(f"torch layernorm bwd dx,dg,db rows={rows} c={c}",
+                     lambda: torch.autograd.grad(y, (xt, gt, bt), dy, retain_graph=True))
+    for m, n in ((16384, 1280), (4096, 2560), (1024, 5120)):
+        hh, dout = h(m, 2 * n), h(m, n)
+        timeit(f"ours  geglu fwd m={m} n={n}", lambda: ops.geglu(hh), bytes_=6.0 * m * n)
+        timeit(f"ours  geglu bwd m={m} n={n}", lambda: ops.geglu_backward(hh, dout), bytes_=10.0 * m * n)
+        ht = hh.clone().requires_grad_()
+        v, g = ht.chunk(2, dim=-1)
+        y = v * F.gelu(g)
+        timeit_eager(f"torch geglu bwd m={m} n={n}", lambda: torch.autograd.grad(y, ht, dout, retain_graph=True),
+                     bytes_=10.0 * m * n)
+
+
 def main():
     which = sys.argv[1] if len(sys.argv) > 1 else "all"
     ops.ensure_device()
+    if which == "norm_bwd":
+        import subprocess
+        smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True).stdout.strip()
+        print(f"GPU: {torch.cuda.get_device_name()} | nvidia-smi: {smi}", flush=True)
+        norm_bwd_cases()
+        return
     if which == "gemm_bwd":
         import subprocess
         smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
