@@ -10,7 +10,9 @@
 //   warp 8     TMA producer: Q once; K tile [BKV][d] and V^T tile [d][BKV] per step, STAGES-deep ring.
 //              Head slices are cut out of the [tokens][heads*d] activations by a 3-D tensor map
 //              (d, heads, tokens) whose innermost extent is d, so the 64-wide box is zero-filled
-//              beyond d — that is the K-dim padding 40->48 / 80->80 / 160->192 for free.
+//              beyond d — that is the K-dim padding 40->48 / 80->80 / 160->192 for free.  V^T is read
+//              through a (key, sample, channel) map whose key extent is the source's n: the keys past n
+//              of a ragged last tile arrive as zeros.  P = 0 masks them, and 0 * NaN would not.
 //   warps 0-7  two warpgroups of 64 query rows each.  Per key tile: S = Q K^T (wgmma, M=64, N=BKV, both
 //              operands in shared memory) into registers; running max / sum in the log2 domain over the
 //              four threads that share a row; P = exp2(S - max) is rounded to fp16 IN REGISTERS, in exactly
@@ -46,7 +48,6 @@ struct AttnKParams {
   long long ldo;
   int nq, n0, n1;
   int kv0_batches, kv1_batches;
-  int ldv0_batch, ldv1_batch;
   int bank_batches;
   float scale_log2;
 };
@@ -101,14 +102,13 @@ __global__ void __launch_bounds__(kWsThreads, MINB)
         const CUtensorMap* tv = src1 ? &p.tmV1 : &p.tmV0;
         const int nsrc = src1 ? p.n1 : p.n0;
         const int kvb = src1 ? (p.kv1_batches > 1 ? b : 0) : (p.kv0_batches > 1 ? b : 0);
-        const int ldvb = src1 ? p.ldv1_batch : p.ldv0_batch;
         const int s = ring_acquire<STAGES>(kv_empty, j);
         mbar_expect_tx(&kv_full[s], C::kStageBytes);
         uint8_t* sk = sKV + s * C::kStageBytes;
         uint8_t* sv = sk + C::kKBytes;
         for (int dc = 0; dc < C::kDkChunks; ++dc)
           tma_load_3d(sk + dc * (BKV * 128), tk, &kv_full[s], dc * 64, head, kvb * nsrc + key0);
-        tma_load_2d(sv, tv, &kv_full[s], kvb * ldvb + key0, head * D);
+        tma_load_3d(sv, tv, &kv_full[s], key0, kvb, head * D);
       }
     }
   } else {
@@ -261,7 +261,7 @@ static int build_and_launch(const mdb_attn_desc* a, float* lse, cudaStream_t st)
     if (r) return r;
     // kDV rows from row head * d: rows past d (d = 40 -> 48) are the next head's or zero-filled, and only feed
     // output columns >= d, which are never stored
-    return tmap_rows(tv, vt, (uint64_t)nb * ldvb, hd, ldvt, 64, kDV);
+    return tmap_vt(tv, vt, n, nb, ldvb, hd, ldvt, kDV);
   };
   if ((rc = mk_kv(a->k0, a->ldk0, a->vt0, a->ldvt0, a->n0, a->kv0_batches, a->ldv0_batch, &kp.tmK0, &kp.tmV0))) return rc;
   if (a->n1 > 0) {
@@ -275,8 +275,6 @@ static int build_and_launch(const mdb_attn_desc* a, float* lse, cudaStream_t st)
   kp.n1 = a->n1;
   kp.kv0_batches = a->kv0_batches;
   kp.kv1_batches = a->kv1_batches;
-  kp.ldv0_batch = a->ldv0_batch;
-  kp.ldv1_batch = a->ldv1_batch;
   kp.bank_batches = a->n1 > 0 ? a->bank_batches : 0;
   kp.scale_log2 = a->scale * 1.4426950408889634f;
   dim3 grid((a->nq + kBQ - 1) / kBQ, a->heads, a->batch);
@@ -323,6 +321,8 @@ int attention_check_desc(const mdb_attn_desc* a) {
   MDB_REQUIRE(a->n1 == 0 || a->kv1_batches == 1 || a->kv1_batches >= a->bank_batches,
               "mdb_attention_f16: kv1_batches must be 1 or cover bank_batches");
   MDB_REQUIRE(a->ldv0_batch >= a->n0 && a->ldv0_batch % 8 == 0, "mdb_attention_f16: ldv0_batch must be >= n0 and %% 8");
+  MDB_REQUIRE(a->n1 == 0 || (a->ldv1_batch >= a->n1 && a->ldv1_batch % 8 == 0),
+              "mdb_attention_f16: ldv1_batch must be >= n1 and %% 8");
   MDB_REQUIRE(a->ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(a->out) & 15) == 0, "mdb_attention_f16: out alignment");
   return MDB_OK;
 }

@@ -120,7 +120,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) attn_bwd_dq_kernel(const __grid
         uint8_t* sk = sKV + s * C::kDqStage;
         for (int dc = 0; dc < C::kDkChunks; ++dc)
           tma_load_3d(sk + dc * C::kChunk64, src ? &p.tmK1 : &p.tmK0, &kv_full[s], dc * 64, head, b * p.n[src] + key0);
-        tma_load_2d(sk + C::kTile64, src ? &p.tmV1 : &p.tmV0, &kv_full[s], b * p.ldv_batch[src] + key0, head * D);
+        tma_load_3d(sk + C::kTile64, src ? &p.tmV1 : &p.tmV0, &kv_full[s], key0, b, head * D);
       }
     }
     return;
@@ -273,8 +273,8 @@ __global__ void __launch_bounds__(kWsThreads, 1) attn_bwd_dkdv_kernel(const __gr
                       b * nsrc + key0 + half * kBwdStep);
       if (kDK)
         for (int half = 0; half < 2; ++half)
-          tma_load_2d(sVt + half * C::kVtBytes, src ? &p.tmV1 : &p.tmV0, &kv_bar,
-                      b * p.ldv_batch[src] + key0 + half * kBwdStep, head * D);
+          tma_load_3d(sVt + half * C::kVtBytes, src ? &p.tmV1 : &p.tmV0, &kv_bar, key0 + half * kBwdStep, b,
+                      head * D);
     }
     for (int j = 0; j < n_qt; ++j) {
       const int s = ring_acquire<STAGES>(q_empty, j);
@@ -434,18 +434,19 @@ static int bwd_launch(const mdb_attn_bwd_desc* a, cudaStream_t st) {
     return tmap_heads(m, base, D, f->heads, rows, ld, kBwdStep);
   };
   // kDV rows from row head * d: rows past d (d = 40 -> 48) are the next head's or zero-filled; they meet only the
-  // zero-filled channels d..47 of the dO tile
-  auto mk_vt = [&](CUtensorMap* m, const void* base, long long ld, long long cols) -> int {
-    return tmap_rows(m, base, cols, hd, ld, 64, C::kDV);
+  // zero-filled channels d..47 of the dO tile.  Keys past n are zero-filled (tmap_vt): dS = P (dP - D) is 0 there
+  // only if dP is finite
+  auto mk_vt = [&](CUtensorMap* m, const void* base, long long ld, int n, int nb, int ldvb) -> int {
+    return tmap_vt(m, base, n, nb, ldvb, hd, ld, C::kDV);
   };
   if ((rc = mk_rows(&kp.tmQ, f->q, f->ldq, (long long)f->batch * f->nq))) return rc;
   if ((rc = mk_rows(&kp.tmDO, a->dout, a->lddout, (long long)f->batch * f->nq))) return rc;
   if ((rc = mk_rows(&kp.tmK0, f->k0, f->ldk0, (long long)f->kv0_batches * f->n0))) return rc;
-  if ((rc = mk_vt(&kp.tmV0, f->vt0, f->ldvt0, (long long)f->kv0_batches * f->ldv0_batch))) return rc;
+  if ((rc = mk_vt(&kp.tmV0, f->vt0, f->ldvt0, f->n0, f->kv0_batches, f->ldv0_batch))) return rc;
   const bool bank = f->n1 > 0 && f->bank_batches > 0;
   if (bank) {
     if ((rc = mk_rows(&kp.tmK1, f->k1, f->ldk1, (long long)f->kv1_batches * f->n1))) return rc;
-    if ((rc = mk_vt(&kp.tmV1, f->vt1, f->ldvt1, (long long)f->kv1_batches * f->ldv1_batch))) return rc;
+    if ((rc = mk_vt(&kp.tmV1, f->vt1, f->ldvt1, f->n1, f->kv1_batches, f->ldv1_batch))) return rc;
   }
   kp.out = static_cast<const __half*>(f->out);
   kp.ldo = f->ldo;
@@ -515,7 +516,6 @@ extern "C" int mdb_attention_bwd_f16(const mdb_attn_bwd_desc* a, mdb_stream_t st
               "would need a reduction across batch elements", f->batch);
   MDB_REQUIRE(a->dout && a->lse && a->dq && a->dk0 && a->dvt0 && a->ws, "mdb_attention_bwd_f16: null operand");
   MDB_REQUIRE(f->n1 == 0 || f->bank_batches == 0 || (a->dk1 && a->dvt1), "mdb_attention_bwd_f16: n1 > 0 needs dk1/dvt1");
-  MDB_REQUIRE(f->n1 == 0 || f->ldv1_batch >= f->n1, "mdb_attention_bwd_f16: ldv1_batch must be >= n1");
   MDB_REQUIRE(a->lddout % 8 == 0 && (reinterpret_cast<uintptr_t>(a->dout) & 15) == 0,
               "mdb_attention_bwd_f16: dout alignment");
   MDB_REQUIRE(a->lddq % 2 == 0 && a->lddk0 % 2 == 0 && a->lddk1 % 2 == 0 &&

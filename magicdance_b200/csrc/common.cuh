@@ -57,6 +57,11 @@ int tmap_rows(CUtensorMap* out, const void* base, uint64_t inner, uint64_t rows,
 // 1 head x box_tokens tokens, zero-filled beyond d
 int tmap_heads(CUtensorMap* out, const void* base, int d, int heads, uint64_t tokens, long long ld,
                uint32_t box_tokens);
+// V^T of attention: `rows` channel rows (row stride ldvt) of nb samples' column blocks of ldvb columns, the first n
+// of each used, as (key, sample, row); boxes of 64 keys x 1 sample x box_rows rows.  Keys >= n are zero-filled, so
+// the padding columns n..ldvb and the next sample's keys never reach shared memory.
+int tmap_vt(CUtensorMap* out, const void* base, int n, int nb, long long ldvb, int rows, long long ldvt,
+            uint32_t box_rows);
 // NHWC images [nb][h][w] of pixels `ld` elements apart, c channels used, as (c, w, h, nb); cs = 2 reads every second
 // pixel along w and h (TMA element strides)
 int tmap_nhwc(CUtensorMap* out, const void* base, int c, int w, int h, int nb, long long ld, const uint32_t box[4],

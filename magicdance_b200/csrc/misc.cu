@@ -88,6 +88,14 @@ int tmap_heads(CUtensorMap* out, const void* base, int d, int heads, uint64_t to
   return make_tmap_f16(out, base, 3, dims, str, box);
 }
 
+int tmap_vt(CUtensorMap* out, const void* base, int n, int nb, long long ldvb, int rows, long long ldvt,
+            uint32_t box_rows) {
+  const uint64_t dims[3] = {(uint64_t)n, (uint64_t)nb, (uint64_t)rows};
+  const uint64_t str[2] = {(uint64_t)ldvb * 2, (uint64_t)ldvt * 2};
+  const uint32_t box[3] = {64, 1, box_rows};
+  return make_tmap_f16(out, base, 3, dims, str, box);
+}
+
 int tmap_nhwc(CUtensorMap* out, const void* base, int c, int w, int h, int nb, long long ld, const uint32_t box[4],
               int cs) {
   const uint64_t dims[4] = {(uint64_t)c, (uint64_t)w, (uint64_t)h, (uint64_t)nb};

@@ -359,7 +359,8 @@ class DenoiseEngine:
         flat = ctx16.reshape(b * n, cd)
         ldv = (n + 7) // 8 * 8
         # tokens padded to ldv per sample with zero rows: ONE swapped-operand GEMM then yields V^T [C, b*ldv] in the
-        # attention kernel's layout (columns n..ldv of each sample stay zero: the kernel masks those keys)
+        # attention kernel's layout.  The kernel never reads columns n..ldv of a sample: its V^T tensor map ends
+        # each sample's keys at n and zero-fills the rest of the ragged tile
         padded = torch.zeros((b, ldv, cd), dtype=torch.float16, device=self.device)
         padded[:, :n].copy_(ctx16)
         padded = padded.reshape(b * ldv, cd)

@@ -156,7 +156,8 @@ def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, re
     """D = epilogue(A @ W^T).  a: [M, K1] fp16 (last dim contiguous, row stride arbitrary) or, with
     conv=(nb, h, w, c), an NHWC activation; w: [N, K] fp16; a2: optional second K-range source.
     splits: 0 = the library picks tile width and split-K (1/2/4/8, reduced inside a thread-block cluster),
-    1 = no split, n = exactly n splits (a count other than 2, 4, 8 goes through an fp32 workspace).
+    1 = no split, n = at most n splits (no split is left empty; a count other than 2, 4, 8 goes through an fp32
+    workspace).
     ln_u: LayerNorm over a's rows folded into the GEMM — w must be W diag(gamma), bias W beta (+ b), ln_u the row sums
     of w (engine.fold_layernorm); D = rstd_r (a w^T - mean_r ln_u) + bias.  Small grids only."""
     lib = _lib.load()
@@ -189,7 +190,9 @@ def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, re
     if TRACE is not None:
         TRACE.append((m, n, k, (tuple(conv) + (conv_stride,)) if conv is not None else None, epilogue, splits,
                       a2.shape[1] if a2 is not None else 0))
-    if splits > 1 and splits not in (2, 4, 8):
+    if splits > 1:
+        # the library rounds the count so that no split is empty (4 splits of 6 K chunks run as 3), and every count
+        # but 2, 4 and 8 reduces through this workspace; with 2, 4 or 8 it reduces in a cluster and ignores it
         ws = _workspace("splitk", splits * m * n, torch.float32, a.device)
         g.splits, g.splitk_ws = splits, ws.data_ptr()
     else:

@@ -8,15 +8,16 @@ from magicdance_b200 import ops
 from tests.kernel_cases import DEV, _rand, rel
 
 
-def attention_bwd_inputs(batch, heads, d, nq, n0, n1=0, ldv_pad=False, seed=0):
+def attention_bwd_inputs(batch, heads, d, nq, n0, n1=0, ldv_pad=False, seed=0, pad=0.0):
     """fp16 operands of a two-source attention in the kernel layouts (vt* transposed, per-batch column blocks of
-    ldv columns), one bank per batch element; also returns V in token-major layout and a gradient of the output."""
+    ldv columns whose padding columns hold `pad`), one bank per batch element; also returns V in token-major layout
+    and a gradient of the output."""
     c = heads * d
     q = _rand(batch * nq, c, seed=seed).half()
     k0 = _rand(batch * n0, c, seed=seed + 1).half()
     v0 = _rand(batch * n0, c, seed=seed + 2).half()
     ldv = (n0 + 7) // 8 * 8 if ldv_pad else n0
-    vt0 = torch.zeros(c, batch * ldv, dtype=torch.float16, device=DEV)
+    vt0 = torch.full((c, batch * ldv), pad, dtype=torch.float16, device=DEV)
     for b in range(batch):
         vt0[:, b * ldv:b * ldv + n0] = v0[b * n0:(b + 1) * n0].t()
     k1 = _rand(batch * n1, c, seed=seed + 3).half() if n1 else None
@@ -47,11 +48,11 @@ def vt_to_tokens(vt, n, ldv, batch):
     return torch.cat([vt[:, b * ldv:b * ldv + n].t() for b in range(batch)], 0)
 
 
-def case_attention_bwd(batch, heads, d, nq, n0, n1=0, bank_batches=None, ldv_pad=False, seed=0):
+def case_attention_bwd(batch, heads, d, nq, n0, n1=0, bank_batches=None, ldv_pad=False, seed=0, pad=0.0):
     """dq, dk0, dv0, dk1, dv1 against torch fp32 autograd; the error is the largest rel-L2 of the five.  Padding
-    columns of dvt0 must stay zero."""
+    columns of dvt0 must stay zero; pad: the value of vt0's padding columns, which must not reach any gradient."""
     bb = batch if bank_batches is None else bank_batches
-    q, k0, v0, vt0, ldv, k1, v1, dout = attention_bwd_inputs(batch, heads, d, nq, n0, n1, ldv_pad, seed)
+    q, k0, v0, vt0, ldv, k1, v1, dout = attention_bwd_inputs(batch, heads, d, nq, n0, n1, ldv_pad, seed, pad)
     kw = dict(heads=heads, d=d, batch=batch, nq=nq, ldv0_batch=ldv)
     if n1:
         kw.update(k1=k1, vt1=v1.t().contiguous(), n1=n1, kv1_batches=batch, bank_batches=bb)
@@ -72,7 +73,8 @@ def case_attention_bwd(batch, heads, d, nq, n0, n1=0, bank_batches=None, ldv_pad
                                    f"ldv={ldv}: rel-L2 dq/dk0/dv0/dk1/dv1 " + " ".join(f"{e:.2e}" for e in errs))
 
 
-# (batch, heads, d, nq, n0[, n1, bank_batches, ldv_pad]); one bank per sample (shared sources are not supported)
+# (batch, heads, d, nq, n0[, n1, bank_batches, ldv_pad, seed, pad]); one bank per sample (shared sources are not
+# supported)
 CASES = [
     (1, 8, 40, 4096, 4096, 4096),      # self + bank at 64x64
     (2, 8, 40, 1024, 1024, 1024),
@@ -87,4 +89,9 @@ CASES = [
     (1, 8, 160, 16, 16, 16),
     (2, 8, 160, 256, 77, 0, None, True),
     (2, 8, 160, 200, 200, 200, 1),     # ragged, and bank_batches < batch
+    # NaN in vt0's padding columns: the dQ kernel's dP = dO V^T must not read them
+    (2, 8, 40, 1024, 77, 0, None, True, 0, float("nan")),
+    (2, 8, 80, 63, 63, 0, None, True, 0, float("nan")),            # nq and n0 below one 64-row step
+    (2, 8, 40, 50, 33, 24, None, True, 0, float("nan")),
+    (1, 8, 160, 33, 40, 16, None, True, 0, float("nan")),
 ]
