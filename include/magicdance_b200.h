@@ -43,7 +43,8 @@ int mdb_device_check(void);
 int64_t mdb_launch_count(void);
 /* sizeof(mdb_gemm_desc) (which = 0) / sizeof(mdb_attn_desc) (which = 1) / sizeof(mdb_attn_bwd_desc) (which = 2) /
  * sizeof(mdb_gemm_bwd_desc) (which = 3) / sizeof(mdb_groupnorm_bwd_desc) (which = 4) /
- * sizeof(mdb_layernorm_bwd_desc) (which = 5): a binding checks its struct mirrors */
+ * sizeof(mdb_layernorm_bwd_desc) (which = 5) / sizeof(mdb_conv3x3_bwd_desc) (which = 6) /
+ * sizeof(mdb_skinny_linear_bwd_desc) (which = 7): a binding checks its struct mirrors */
 int64_t mdb_abi_struct_bytes(int32_t which);
 
 /* Launch heuristics, process-wide (defaults in parentheses); tests use the setter to force a kernel variant onto small
@@ -301,6 +302,37 @@ int mdb_conv3x3_direct_f16(const void* x, const void* wt, const float* bias, con
                            int32_t batch, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t stride,
                            int32_t silu, mdb_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Backward of mdb_conv3x3_direct_f16: the differentiation of the ControlNet hint encoder (cldm.py:599-615), the 4->320
+ * input conv (openaimodel.py:554-558) and the 320->4 output conv (openaimodel.py:744-748).  With z = conv(x) + bias,
+ * y = act(z) + residual and dz = dy silu'(z) (dy without SiLU):
+ *   dx = the transposed conv of dz, dW[o][i][kh][kw] = sum_pix dz_o x_i(shifted), dbias = sum_pix dz.
+ * z is recomputed by the forward kernel (silu = 0) into the workspace; the forward's own output is never changed.
+ * Stride 1: dx is the forward kernel applied to dz with wt_t, the flipped and transposed weight
+ * wt_t[i][kh][kw][o] = wt[o][2-kh][2-kw][i] (at most a few hundred KB; the caller relayouts it).  Stride 2: dx by a
+ * gather over the 1, 2 or 4 taps each input pixel's parity admits (any h, w).  dW / dbias: per-CTA fp32 slabs summed
+ * in a fixed order, no atomics: two calls give bit-equal results.  The residual's gradient is dy itself.
+ *   x, wt, bias, batch, h, w, cin, cout, stride, silu : the forward's arguments (bias may be NULL)
+ *   dy     : fp16 NHWC [B][ho][wo][cout], ho = (h-1)/stride+1
+ *   dx     : fp16 NHWC [B][h][w][cin], overwritten; NULL = not wanted (the first hint conv's input is the pose map)
+ *   dw     : fp32 [cout][cin][3][3] (the Conv2d parameter's own OIHW layout); dbias: fp32 [cout]; NULL = not wanted;
+ *            *_accumulate != 0 adds into the destination instead of overwriting it
+ *   ws     : fp32 workspace of mdb_conv3x3_direct_bwd_ws_floats(desc) floats (no initial value needed)
+ * x, wt, wt_t, dy, dx and ws are 16-byte aligned.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct mdb_conv3x3_bwd_desc {
+  const void* x; const void* wt; const void* wt_t; const float* bias; const void* dy;
+  int32_t batch; int32_t h; int32_t w; int32_t cin; int32_t cout; int32_t stride; int32_t silu;
+  void* dx;
+  float* dw; int32_t dw_accumulate;
+  float* dbias; int32_t dbias_accumulate;
+  float* ws;
+} mdb_conv3x3_bwd_desc;
+
+int mdb_conv3x3_direct_bwd_f16(const mdb_conv3x3_bwd_desc* desc, mdb_stream_t stream);
+/* workspace floats mdb_conv3x3_direct_bwd_f16 needs for this descriptor; negative MDB_ERR_* for one it rejects */
+int64_t mdb_conv3x3_direct_bwd_ws_floats(const mdb_conv3x3_bwd_desc* desc);
+
 /* im2col for 3x3 pad-1 convolutions, stride 1 or 2: x NHWC [B][h][w][c] -> col [B*ho*wo][9*c] with K order
  * (kh, kw, c), ho = (h-1)/stride+1, consumed by mdb_gemm_f16.  Used for Downsample.op (stride 2,
  * openaimodel.py:154-180) and as the general path for latent sizes whose rows do not tile into the
@@ -316,6 +348,10 @@ int mdb_im2col3x3_br_f16(const void* x, void* col, int32_t batch, int32_t h, int
 
 /* nearest x2 upsample (Upsample.forward, openaimodel.py:129-139): NHWC [B][h][w][c] -> [B][2h][2w][c] */
 int mdb_upsample2x_f16(const void* x, void* y, int32_t batch, int32_t h, int32_t w, int32_t c, mdb_stream_t stream);
+/* its backward: dx[B][h][w][c] (+)= the sum of each 2x2 block of dy [B][2h][2w][c] (fp16), in a fixed order;
+ * dx_dtype MDB_DTYPE_F16 | MDB_DTYPE_F32, accumulate != 0 adds into dx.  c % 8 == 0, 16-byte aligned pointers. */
+int mdb_upsample2x_bwd_f16(const void* dy, void* dx, int32_t dx_dtype, int32_t accumulate, int32_t batch, int32_t h,
+                           int32_t w, int32_t c, mdb_stream_t stream);
 
 /* y = a + b (b broadcast over the batch when b_batches == 1); the ControlNet residual adds
  * `h += pose_control.pop()` / `hs.pop() + pose_control.pop()` (cldm.py:93-104). n = elements per batch */
@@ -333,6 +369,28 @@ int mdb_timestep_embedding_f32(const int64_t* t, int32_t t_count, float* out, in
  * stacking their weights along n.  silu_out applies SiLU to the result (time_embed's middle SiLU). */
 int mdb_skinny_linear_f32(const float* x, const void* w, const float* bias, float* out, int32_t rows, int32_t n,
                           int32_t k, int32_t silu_in, int32_t silu_out, mdb_stream_t stream);
+
+/* Backward of mdb_skinny_linear_f32 without silu_out (training runs time_embed.0 with silu_out = 0 and time_embed.2
+ * with silu_in = 1, which is bit-identical to the fused forward and keeps the pre-activation):
+ *   dx[r][k]  = sum_n dy[r][n] W[n][k]  (* silu'(x[r][k]) when silu_in),
+ *   dw[n][k]  = sum_r dy[r][n] f(x[r][k]),  dbias[n] = sum_r dy[r][n]   (f = SiLU when silu_in), all fp32.
+ * Deterministic: dx sums per-chunk fp32 slabs over n in chunk order; dw / dbias sum the rows in row order.  Inputs
+ * taller than 16 rows go through in row chunks: dx per chunk, dw / dbias of later chunks with *_accumulate = 1.
+ *   x, w, rows, n, k, silu_in : the forward's arguments (rows 1..16, k % 8 == 0); dy fp32 [rows][n]
+ *   dx fp32 [rows][k], dw fp32 [n][k], dbias fp32 [n]: NULL = not wanted; *_accumulate as above
+ *   ws     : fp32 workspace of mdb_skinny_linear_bwd_ws_floats(desc) floats (no initial value needed)
+ * x, w, dy, dx, dw and ws are 16-byte aligned. */
+typedef struct mdb_skinny_linear_bwd_desc {
+  const float* x; const void* w; const float* dy;
+  int32_t rows; int32_t n; int32_t k; int32_t silu_in;
+  float* dx; int32_t dx_accumulate;
+  float* dw; int32_t dw_accumulate;
+  float* dbias; int32_t dbias_accumulate;
+  float* ws;
+} mdb_skinny_linear_bwd_desc;
+
+int mdb_skinny_linear_bwd_f32(const mdb_skinny_linear_bwd_desc* desc, mdb_stream_t stream);
+int64_t mdb_skinny_linear_bwd_ws_floats(const mdb_skinny_linear_bwd_desc* desc);
 
 
 /* Row softmax in place over fp16 logits x[rows][cols] (row pitch ld elements), fp32 arithmetic:

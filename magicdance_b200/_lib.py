@@ -86,6 +86,29 @@ class LayerNormBwdDesc(C.Structure):
     ]
 
 
+class Conv3x3BwdDesc(C.Structure):
+    _fields_ = [
+        ("x", c_void_p), ("wt", c_void_p), ("wt_t", c_void_p), ("bias", c_void_p), ("dy", c_void_p),
+        ("batch", c_int32), ("h", c_int32), ("w", c_int32), ("cin", c_int32), ("cout", c_int32), ("stride", c_int32),
+        ("silu", c_int32),
+        ("dx", c_void_p),
+        ("dw", c_void_p), ("dw_accumulate", c_int32),
+        ("dbias", c_void_p), ("dbias_accumulate", c_int32),
+        ("ws", c_void_p),
+    ]
+
+
+class SkinnyBwdDesc(C.Structure):
+    _fields_ = [
+        ("x", c_void_p), ("w", c_void_p), ("dy", c_void_p),
+        ("rows", c_int32), ("n", c_int32), ("k", c_int32), ("silu_in", c_int32),
+        ("dx", c_void_p), ("dx_accumulate", c_int32),
+        ("dw", c_void_p), ("dw_accumulate", c_int32),
+        ("dbias", c_void_p), ("dbias_accumulate", c_int32),
+        ("ws", c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/magicdance_b200.h declares
 SIGNATURES = {
     "mdb_abi_version": (c_int32, []),
@@ -115,13 +138,19 @@ SIGNATURES = {
                                     c_void_p]),
     "mdb_conv3x3_direct_f16": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
                                          c_int32, c_int32, c_int32, c_int32, c_void_p]),
+    "mdb_conv3x3_direct_bwd_f16": (c_int32, [C.POINTER(Conv3x3BwdDesc), c_void_p]),
+    "mdb_conv3x3_direct_bwd_ws_floats": (c_int64, [C.POINTER(Conv3x3BwdDesc)]),
     "mdb_im2col3x3_f16": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p]),
     "mdb_im2col3x3_br_f16": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p]),
     "mdb_upsample2x_f16": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p]),
+    "mdb_upsample2x_bwd_f16": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                         c_void_p]),
     "mdb_add_f16": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p]),
     "mdb_timestep_embedding_f32": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p]),
     "mdb_skinny_linear_f32": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
                                         c_int32, c_void_p]),
+    "mdb_skinny_linear_bwd_f32": (c_int32, [C.POINTER(SkinnyBwdDesc), c_void_p]),
+    "mdb_skinny_linear_bwd_ws_floats": (c_int64, [C.POINTER(SkinnyBwdDesc)]),
     "mdb_nchw_f32_to_nhwc_f16": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p]),
     "mdb_nhwc_f16_to_nchw_f32": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p]),
     "mdb_softmax_rows_f16": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_float, c_void_p]),
@@ -162,7 +191,7 @@ def load():
         raise RuntimeError(f"magicdance_b200: ABI version mismatch ({lib.mdb_abi_version()} != {ABI_VERSION}); "
                            "rebuild the library")
     for which, mirror in ((0, GemmDesc), (1, AttnDesc), (2, AttnBwdDesc), (3, GemmBwdDesc), (4, GroupNormBwdDesc),
-                          (5, LayerNormBwdDesc)):
+                          (5, LayerNormBwdDesc), (6, Conv3x3BwdDesc), (7, SkinnyBwdDesc)):
         if lib.mdb_abi_struct_bytes(which) != C.sizeof(mirror):
             raise RuntimeError(f"magicdance_b200: {mirror.__name__} mirrors {C.sizeof(mirror)} bytes, the library's "
                                f"struct has {lib.mdb_abi_struct_bytes(which)}: the binding and the library disagree")

@@ -15,7 +15,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIB_DIR = os.path.join(PKG, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libmagicdance_b200.so")
 STAMP = os.path.join(LIB_DIR, "build.stamp")
-SOURCES = ["gemm.cu", "gemm_bwd.cu", "attention.cu", "attention_bwd.cu", "norm.cu", "norm_bwd.cu", "misc.cu"]
+SOURCES = ["gemm.cu", "gemm_bwd.cu", "attention.cu", "attention_bwd.cu", "norm.cu", "norm_bwd.cu", "conv_bwd.cu", "misc.cu"]
 HEADERS = ["common.cuh", "wgmma.cuh", "norm.cuh", os.path.join("..", "..", "include", "magicdance_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

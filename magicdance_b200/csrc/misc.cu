@@ -560,6 +560,10 @@ extern "C" int64_t mdb_abi_struct_bytes(int32_t which) {
       return (int64_t)sizeof(mdb_groupnorm_bwd_desc);
     case 5:
       return (int64_t)sizeof(mdb_layernorm_bwd_desc);
+    case 6:
+      return (int64_t)sizeof(mdb_conv3x3_bwd_desc);
+    case 7:
+      return (int64_t)sizeof(mdb_skinny_linear_bwd_desc);
     default:
       return -1;
   }

@@ -812,3 +812,253 @@ def cfg_ddim_update(x, eps_c, eps_u, coef, noise=None, x_prev=None, pred_x0=None
                "cfg_ddim_update_f32")
     return x_prev, pred_x0
 
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Backward of the direct 3x3 conv, the skinny timestep Linear and the nearest x2 upsample (csrc/conv_bwd.cu), and the
+# autograd ops over them and over the layout converts.
+# ---------------------------------------------------------------------------------------------------------------------
+def flip_conv_weight(wt, *, cin, cout):
+    """[cout][3][3][cin] -> [cin][2-kh][2-kw][cout] fp16: the weight of the stride-1 dx conv (weight-sized relayout)"""
+    return wt.reshape(cout, 3, 3, cin).flip(1, 2).permute(3, 1, 2, 0).contiguous().reshape(cin, 9 * cout)
+
+
+def _vec_out(t, n, dtype, device, name):
+    """a contiguous gradient destination of n elements: `t` or a new tensor"""
+    if t is None:
+        t = torch.empty(n, dtype=dtype, device=device)
+    _chk(t, dtype, name)
+    assert t.is_contiguous() and t.numel() == n, (name, t.shape, n)
+    return t
+
+
+def conv3x3_direct_backward(x, wt, dy, *, batch, h, w, cin, cout, stride=1, bias=None, silu=False, wt_t=None,
+                            grads=("x", "w", "bias"), out_dx=None, out_dw=None, out_dbias=None, accumulate=()):
+    """Gradients of y = conv3x3_direct(x, wt, bias, batch=, h=, w=, cin=, cout=, stride=, silu=[, residual=]) from
+    dy = dL/dy (fp16 [B*ho*wo, cout]), csrc/conv_bwd.cu; with SiLU the pre-activation is recomputed by the forward
+    kernel.  `grads` names the gradients to compute among "x" (fp16 [B*h*w, cin], overwritten), "w" (fp32
+    [cout, cin, 3, 3], the Conv2d parameter's OIHW layout) and "bias" (fp32 [cout]); each goes to its out_* tensor
+    when given, and names in `accumulate` ("w", "bias") add into it.  wt_t: flip_conv_weight(wt), made here when
+    None and needed (stride-1 dx).  The residual's gradient is dy.  Returns (dx, dw, dbias).  Deterministic."""
+    lib = _lib.load()
+    _chk(x, torch.float16, "x")
+    _chk(wt, torch.float16, "wt")
+    _chk(dy, torch.float16, "dy")
+    assert x.is_contiguous() and wt.is_contiguous() and dy.is_contiguous()
+    acc = set(accumulate)
+    if "x" in acc:
+        raise RuntimeError("magicdance_b200.conv3x3_direct_backward: dx is always overwritten (no accumulation)")
+    dev = x.device
+    d = _lib.Conv3x3BwdDesc()
+    d.x, d.wt, d.dy = x.data_ptr(), wt.data_ptr(), dy.data_ptr()
+    if bias is not None:
+        _chk(bias, torch.float32, "bias")
+        d.bias = bias.data_ptr()
+    d.batch, d.h, d.w, d.cin, d.cout, d.stride, d.silu = batch, h, w, cin, cout, stride, int(silu)
+    dx = dw = dbias = None
+    if "x" in grads:
+        if stride == 1:
+            wt_t = flip_conv_weight(wt, cin=cin, cout=cout) if wt_t is None else wt_t
+            _chk(wt_t, torch.float16, "wt_t")
+            assert wt_t.is_contiguous() and wt_t.numel() == wt.numel()
+            d.wt_t = wt_t.data_ptr()
+        dx = torch.empty((batch * h * w, cin), dtype=torch.float16, device=dev) if out_dx is None else out_dx
+        _chk(dx, torch.float16, "out_dx")
+        assert dx.is_contiguous() and tuple(dx.shape) == (batch * h * w, cin), dx.shape
+        d.dx = dx.data_ptr()
+    if "w" in grads:
+        dw = out_dw if out_dw is not None else torch.empty((cout, cin, 3, 3), dtype=torch.float32, device=dev)
+        _vec_out(dw, cout * cin * 9, torch.float32, dev, "out_dw")
+        d.dw, d.dw_accumulate = dw.data_ptr(), "w" in acc
+    if "bias" in grads:
+        dbias = _vec_out(out_dbias, cout, torch.float32, dev, "out_dbias")
+        d.dbias, d.dbias_accumulate = dbias.data_ptr(), "bias" in acc
+    need = int(lib.mdb_conv3x3_direct_bwd_ws_floats(C.byref(d)))
+    if need < 0:
+        _lib.check(need, "conv3x3_direct_bwd_f16")
+    d.ws = _workspace("conv_bwd", need, torch.float32, dev).data_ptr()
+    _lib.check(lib.mdb_conv3x3_direct_bwd_f16(C.byref(d), _stream()), "conv3x3_direct_bwd_f16")
+    return dx, dw, dbias
+
+
+class DirectConv3x3(torch.autograd.Function):
+    """conv3x3_direct() as an autograd op: an fp16 gradient to x, fp32 ones to the OIHW parameter w_param (passed with
+    its fp16 packed copy wt) and to the bias, dy to the residual.  Only the gradients autograd asks for are computed.
+    Positional arguments in direct_conv3x3()'s order."""
+
+    @staticmethod
+    def forward(ctx, x, wt, w_param, bias, residual, batch, h, w, cin, cout, stride, silu):
+        ctx.kw = dict(batch=batch, h=h, w=w, cin=cin, cout=cout, stride=stride, silu=silu)
+        ctx.save_for_backward(x, wt, w_param, bias)
+        ctx.has_residual = residual is not None
+        return conv3x3_direct(x, wt, bias, residual=residual, **ctx.kw)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, wt, w_param, bias = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        grads = [nm for nm, want in (("x", need[0]), ("w", need[1] or need[2]), ("bias", need[3])) if want]
+        dy = dy.contiguous()
+        dx = dw = dbias = None
+        if grads:
+            dx, dw, dbias = conv3x3_direct_backward(x, wt, dy, bias=bias, grads=grads, **ctx.kw)
+        g_wt = g_wp = None
+        if dw is not None:
+            if w_param is not None:
+                g_wp = dw.view(w_param.shape)
+            else:
+                g_wt = dw.permute(0, 2, 3, 1).reshape(wt.shape).to(wt.dtype)
+        return dx, g_wt, g_wp, dbias, dy if ctx.has_residual else None, *(None,) * 7
+
+
+def direct_conv3x3(x, wt, *, batch, h, w, cin, cout, stride=1, silu=False, w_param=None, bias=None, residual=None):
+    """Differentiable conv3x3_direct() (DirectConv3x3): x NHWC fp16 [B*h*w, cin], wt fp16 [cout][3][3][cin] (packed
+    from the fp32 OIHW w_param, which receives the weight gradient), bias fp32 [cout], residual fp16 like the output."""
+    return DirectConv3x3.apply(x, wt, w_param, bias, residual, batch, h, w, cin, cout, stride, silu)
+
+
+def skinny_linear_backward(x, w, dy, *, silu_in=False, grads=("x", "w", "bias"), out_dx=None, out_dw=None,
+                           out_dbias=None, accumulate=()):
+    """Gradients of out = skinny_linear(x, w, bias, silu_in=) (silu_out off) from dy (fp32 [rows, n]),
+    csrc/conv_bwd.cu: dx fp32 [rows, k] (times silu'(x) with silu_in), dw fp32 [n, k], dbias fp32 [n].  grads / out_* /
+    accumulate ("x", "w", "bias") as in gemm_backward.  Inputs taller than SKINNY_MAX_ROWS go through in row chunks, as
+    in the forward; dw and dbias of later chunks add onto earlier ones, so the row order of the sums is fixed.
+    Returns (dx, dw, dbias).  Deterministic."""
+    lib = _lib.load()
+    _chk(x, torch.float32, "x")
+    _chk(w, torch.float16, "w")
+    _chk(dy, torch.float32, "dy")
+    rows, k = x.shape
+    n = w.shape[0]
+    assert w.shape[1] == k and tuple(dy.shape) == (rows, n), (x.shape, w.shape, dy.shape)
+    assert x.is_contiguous() and w.is_contiguous() and dy.is_contiguous()
+    dev = x.device
+    acc = set(accumulate)
+    dx = dw = dbias = None
+    if "x" in grads:
+        dx = _grad_out(out_dx, (rows, k), torch.float32, dev, "out_dx")
+        _chk(dx, torch.float32, "out_dx")
+        assert dx.is_contiguous()
+    if "w" in grads:
+        dw = _grad_out(out_dw, (n, k), torch.float32, dev, "out_dw")
+        _chk(dw, torch.float32, "out_dw")
+        assert dw.is_contiguous()
+    if "bias" in grads:
+        dbias = _vec_out(out_dbias, n, torch.float32, dev, "out_dbias")
+    for r0 in range(0, rows, SKINNY_MAX_ROWS):
+        d = _lib.SkinnyBwdDesc()
+        d.x, d.w, d.dy = x[r0:].data_ptr(), w.data_ptr(), dy[r0:].data_ptr()
+        d.rows, d.n, d.k, d.silu_in = min(SKINNY_MAX_ROWS, rows - r0), n, k, int(silu_in)
+        if dx is not None:
+            d.dx, d.dx_accumulate = dx[r0:].data_ptr(), "x" in acc
+        if dw is not None:
+            d.dw, d.dw_accumulate = dw.data_ptr(), r0 > 0 or "w" in acc
+        if dbias is not None:
+            d.dbias, d.dbias_accumulate = dbias.data_ptr(), r0 > 0 or "bias" in acc
+        need = int(lib.mdb_skinny_linear_bwd_ws_floats(C.byref(d)))
+        if need < 0:
+            _lib.check(need, "skinny_linear_bwd_f32")
+        d.ws = _workspace("skinny_bwd", need, torch.float32, dev).data_ptr()
+        _lib.check(lib.mdb_skinny_linear_bwd_f32(C.byref(d), _stream()), "skinny_linear_bwd_f32")
+    return dx, dw, dbias
+
+
+class SkinnyLinear(torch.autograd.Function):
+    """skinny_linear() (silu_out off) as an autograd op: fp32 gradients to x, to the fp32 parameter w_param (passed with
+    its fp16 copy w, layout (out, in)) and to the bias.  Positional arguments in skinny_linear_ad()'s order."""
+
+    @staticmethod
+    def forward(ctx, x, w, w_param, bias, silu_in):
+        ctx.save_for_backward(x, w, w_param)
+        ctx.silu_in = silu_in
+        return skinny_linear(x, w, bias, silu_in=silu_in)
+
+    @staticmethod
+    def backward(ctx, dout):
+        x, w, w_param = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        grads = [nm for nm, want in (("x", need[0]), ("w", need[1] or need[2]), ("bias", need[3])) if want]
+        dx = dw = dbias = None
+        if grads:
+            dx, dw, dbias = skinny_linear_backward(x, w, dout.contiguous(), silu_in=ctx.silu_in, grads=grads)
+        g_w = g_wp = None
+        if dw is not None:
+            if w_param is not None:
+                g_wp = dw.view(w_param.shape)
+            else:
+                g_w = dw.to(w.dtype)
+        return dx, g_w, g_wp, dbias, None
+
+
+def skinny_linear_ad(x, w, bias=None, *, w_param=None, silu_in=False):
+    """Differentiable skinny_linear() (SkinnyLinear): x fp32 [rows, k], w fp16 [n, k] (the copy of the fp32 w_param),
+    bias fp32 [n].  Training runs time_embed.0 plain and time_embed.2 with silu_in, bit-identical to the fused
+    silu_out forward."""
+    return SkinnyLinear.apply(x, w, w_param, bias, silu_in)
+
+
+def upsample2x_backward(dy, *, batch, h, w, c, dx_dtype=torch.float16, out_dx=None, accumulate=False):
+    """Gradient of y = upsample2x(x, batch=, h=, w=, c=) from dy (fp16 [B*2h*2w, c]): dx [B*h*w, c] = the 2x2 block
+    sums, fp16 or fp32 (out_dx's dtype when given); accumulate adds into out_dx."""
+    lib = _lib.load()
+    _chk(dy, torch.float16, "dy")
+    assert dy.is_contiguous() and tuple(dy.shape) == (batch * 4 * h * w, c), dy.shape
+    dx = _grad_out(out_dx, (batch * h * w, c), dx_dtype, dy.device, "out_dx")
+    assert dx.is_contiguous()
+    _lib.check(lib.mdb_upsample2x_bwd_f16(dy.data_ptr(), dx.data_ptr(), _DTYPES[dx.dtype], int(accumulate), batch, h,
+                                          w, c, _stream()), "upsample2x_bwd_f16")
+    return dx
+
+
+class Upsample2x(torch.autograd.Function):
+    """upsample2x() (nearest x2, NHWC fp16) as an autograd op: the gradient is the 2x2 block sum."""
+
+    @staticmethod
+    def forward(ctx, x, batch, h, w, c):
+        ctx.kw = dict(batch=batch, h=h, w=w, c=c)
+        return upsample2x(x, **ctx.kw)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return upsample2x_backward(dy.contiguous(), **ctx.kw), None, None, None, None
+
+
+def upsample_2x(x, *, batch, h, w, c):
+    """Differentiable upsample2x() (Upsample2x): x fp16 [B*h*w, c] -> [B*2h*2w, c]."""
+    return Upsample2x.apply(x, batch, h, w, c)
+
+
+class NchwToNhwc(torch.autograd.Function):
+    """nchw_f32_to_nhwc_f16() (one copy) as an autograd op; the gradient is the opposite convert."""
+
+    @staticmethod
+    def forward(ctx, x):
+        ctx.shape = tuple(x.shape)
+        return nchw_f32_to_nhwc_f16(x)
+
+    @staticmethod
+    def backward(ctx, dy):
+        b, c, h, w = ctx.shape
+        return nhwc_f16_to_nchw_f32(dy.contiguous(), batch=b, c=c, h=h, w=w)
+
+
+def nchw_to_nhwc(x):
+    """Differentiable nchw_f32_to_nhwc_f16() (NchwToNhwc): NCHW fp32 -> NHWC fp16 [B*H*W, C]."""
+    return NchwToNhwc.apply(x)
+
+
+class NhwcToNchw(torch.autograd.Function):
+    """nhwc_f16_to_nchw_f32() as an autograd op; the gradient is the opposite convert."""
+
+    @staticmethod
+    def forward(ctx, x, batch, c, h, w):
+        return nhwc_f16_to_nchw_f32(x, batch=batch, c=c, h=h, w=w)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return nchw_f32_to_nhwc_f16(dy.contiguous()), None, None, None, None
+
+
+def nhwc_to_nchw(x, *, batch, c, h, w):
+    """Differentiable nhwc_f16_to_nchw_f32() (NhwcToNchw): NHWC fp16 [B*H*W, C] -> NCHW fp32."""
+    return NhwcToNchw.apply(x, batch, c, h, w)

@@ -196,9 +196,74 @@ def norm_bwd_cases():
                      bytes_=10.0 * m * n)
 
 
+def direct_bwd_cases():
+    """our direct-conv backward against cuDNN's convolution_backward (fp16, channels-last) on the same tensors, our
+    skinny-Linear backward against torch's fp32 matmuls, and our upsample backward, at the training shapes (4 samples,
+    512^2 pose maps, 64^2 latent).  Conv FLOP are algorithmic (2 M N K per gradient); the SiLU rows include the
+    recomputed forward.  Skinny bytes: W read once (fp16) plus dW written (fp32); upsample: dy read + dx written."""
+    from tests.direct_bwd_cases import HINT_LAYERS
+    b, s = 4, 512
+    convs = [(cin, cout, st, s // div, True) for cin, cout, st, div in HINT_LAYERS] + [(4, 320, 1, 64, False),
+                                                                                        (320, 4, 1, 64, False)]
+    for cin, cout, st, hw, silu in convs:
+        ho = (hw - 1) // st + 1
+        x, wt, dy, bias = h(b * hw * hw, cin), h(cout, 9 * cin) * 0.1, h(b * ho * ho, cout), f(cout)
+        fl = 2.0 * b * ho * ho * cout * 9 * cin
+        tag = f"B={b} {hw}x{hw} {cin}->{cout} s{st}"
+        kw = dict(batch=b, h=hw, w=hw, cin=cin, cout=cout, stride=st, bias=bias)
+        wt_t = ops.flip_conv_weight(wt, cin=cin, cout=cout)
+        dw, db = torch.empty(cout, cin, 3, 3, device=D), torch.empty(cout, device=D)
+        dx = torch.empty(b * hw * hw, cin, dtype=torch.float16, device=D)
+        if cin != 3:
+            timeit(f"ours  dx      {tag}", lambda: ops.conv3x3_direct_backward(x, wt, dy, grads=("x",), wt_t=wt_t,
+                                                                                out_dx=dx, **kw), flops=fl)
+        timeit(f"ours  dW,db   {tag}", lambda: ops.conv3x3_direct_backward(x, wt, dy, grads=("w", "bias"), out_dw=dw,
+                                                                            out_dbias=db, **kw), flops=fl)
+        grads = ("w", "bias") if cin == 3 else ("x", "w", "bias")
+        timeit(f"ours  all{'+silu' if silu else '     '} {tag}",
+               lambda: ops.conv3x3_direct_backward(x, wt, dy, grads=grads, wt_t=wt_t, silu=silu, out_dx=dx,
+                                                   out_dw=dw, out_dbias=db, **kw), flops=fl * len(grads[:2]))
+        xc = x.view(b, hw, hw, cin).permute(0, 3, 1, 2)  # NCHW views of NHWC memory: channels-last
+        wc = wt.view(cout, 3, 3, cin).permute(0, 3, 1, 2).contiguous(memory_format=torch.channels_last)
+        g = dy.view(b, ho, ho, cout).permute(0, 3, 1, 2)
+        cb = lambda mask: torch.ops.aten.convolution_backward(g, xc, wc, [cout], [st] * 2, [1, 1], [1, 1], False,
+                                                              [0, 0], 1, mask)
+        if cin != 3:
+            timeit_eager(f"cudnn dx      {tag}", lambda: cb([True, False, False]), flops=fl)
+        timeit_eager(f"cudnn dW,db   {tag}", lambda: cb([False, True, True]), flops=fl)
+        timeit_eager(f"cudnn all     {tag}", lambda: cb([cin != 3, True, True]), flops=fl * len(grads[:2]))
+    for rows, n, k, silu in ((4, 20160, 1280, True), (4, 9600, 1280, True), (4, 1280, 320, False),
+                             (4, 1280, 1280, True)):
+        x, w, dy = f(rows, k), h(n, k) * 0.03, f(rows, n)
+        dx, dw, db = torch.empty(rows, k, device=D), torch.empty(n, k, device=D), torch.empty(n, device=D)
+        tag = f"rows={rows} n={n} k={k}"
+        timeit(f"ours  skinny dx,dW,db {tag}",
+               lambda: ops.skinny_linear_backward(x, w, dy, silu_in=silu, out_dx=dx, out_dw=dw, out_dbias=db),
+               bytes_=6.0 * n * k)
+        w32 = w.float()
+        timeit_eager(f"torch linear dx,dW,db (fp32 mm) {tag}", lambda: (dy @ w32, dy.t() @ x, dy.sum(0)),
+                     bytes_=8.0 * n * k)
+    for hw, c in ((8, 1280), (16, 1280), (32, 640)):
+        dy = h(b * 4 * hw * hw, c)
+        e = b * hw * hw * c
+        timeit(f"ours  upsample2x bwd B={b} {hw}x{hw}->{2 * hw} c={c}",
+               lambda: ops.upsample2x_backward(dy, batch=b, h=hw, w=hw, c=c), bytes_=10.0 * e)
+        dyt = dy.view(b, 2 * hw, 2 * hw, c).permute(0, 3, 1, 2)
+        timeit_eager(f"torch upsample_nearest2d bwd B={b} {hw}x{hw}->{2 * hw} c={c}",
+                     lambda: torch.ops.aten.upsample_nearest2d_backward(dyt, [2 * hw, 2 * hw], [b, c, hw, hw]),
+                     bytes_=10.0 * e)
+
+
 def main():
     which = sys.argv[1] if len(sys.argv) > 1 else "all"
     ops.ensure_device()
+    if which == "direct_bwd":
+        import subprocess
+        smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True).stdout.strip()
+        print(f"GPU: {torch.cuda.get_device_name()} | nvidia-smi: {smi}", flush=True)
+        direct_bwd_cases()
+        return
     if which == "norm_bwd":
         import subprocess
         smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
