@@ -14,7 +14,7 @@ from __future__ import annotations
 
 import torch
 
-from .. import ops
+from .. import ops, train
 from ..engine import DenoiseEngine
 from .ddpm import LatentDiffusionReferenceOnly
 from .modules import UNetModel
@@ -104,8 +104,18 @@ class ControlLDMReferenceOnlyPose(LatentDiffusionReferenceOnly):
             self._engine_nets = packed
         return self._engine
 
+    def _nets(self):
+        return self.model.diffusion_model, self.appearance_control_model, self.pose_control_model
+
+    def wants_grad(self, x_noisy):
+        """Does this call build a graph?  Grad mode on, and x_noisy or any parameter of the three nets requires grad."""
+        if not torch.is_grad_enabled():
+            return False
+        return x_noisy.requires_grad or any(p.requires_grad for n in self._nets() for p in n.parameters())
+
     def apply_model(self, x_noisy, t, cond, reference_image_noisy, uc=False, *args, **kwargs):
-        """cldm.py:1099-1117 — same arguments, returns eps (B,4,h,w) fp32."""
+        """cldm.py:1099-1117 — same arguments, returns eps (B,4,h,w) fp32.  Differentiable (magicdance_b200.train)
+        when grad mode is on and something requires grad; the inference engine otherwise."""
         assert isinstance(cond, dict)
         assert not self.only_mid_control
         cond_txt = _one(cond["c_crossattn"])
@@ -113,6 +123,13 @@ class ControlLDMReferenceOnlyPose(LatentDiffusionReferenceOnly):
             raise NotImplementedError("c_crossattn_void is never passed by the MagicPose scripts")
         assert self.control_enabled and cond.get("c_concat") is not None, "the pose map (c_concat) is required"
         cond_hint = _one(cond["c_concat"])
+        if not uc and self.wants_grad(x_noisy):
+            nets = self._nets()
+            eps = train.apply_model(*nets, x_noisy, t, cond_txt, cond_hint, reference_image_noisy)
+            for n in nets:  # an optimizer step will change these weights, maybe without bumping version counters
+                if any(p.requires_grad for p in n.parameters()):
+                    n.invalidate()
+            return eps
         eng = self.engine(x_noisy.device)
         return eng.apply_model(x_noisy, t, cond_txt, cond_hint, reference_image_noisy, uc=uc)
 

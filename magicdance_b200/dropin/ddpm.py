@@ -1,7 +1,7 @@
 """Drop-in for the parts of model_lib/ControlNet/ldm/models/diffusion/ddpm.py the hot path's callers
 touch: DiffusionWrapper (ddpm.py:1313-1352), the DDPM noise-schedule buffers (ddpm.py:120-191) and
 LatentDiffusionReferenceOnly (ddpm.py:1803-2601): q_sample, forward/p_losses (the training entry
-point — forward value only, see below), sample_log, the first-/cond-stage plumbing.
+point, see below), sample_log, the first-/cond-stage plumbing.
 
 Scope (SURVEY §8): this is host-side caller code and stays Python.  pytorch_lightning is not needed
 (the reference only uses LightningModule as an nn.Module with a .device property on this path).
@@ -9,9 +9,11 @@ The VAE and the CLIP text encoder are NOT part of the accelerated path: they are
 the YAML with whatever classes the `target:` strings resolve to (the reference's own, when its tree is
 importable); when they cannot be imported the corresponding methods raise a clear error.
 
-Training: p_losses reproduces the reference's loss VALUE (same signature, same loss_dict keys) through
-the CUDA kernels, but the kernels have no backward yet (SURVEY §8f rank 3), so it runs under no_grad
-and refuses to pretend otherwise when a gradient is requested.
+Training: p_losses returns the reference's loss (same signature, same loss_dict keys) through the CUDA
+kernels.  When grad mode is on and a parameter of the three networks (or x_noisy) requires grad,
+ControlLDMReferenceOnlyPose.apply_model runs the differentiable forward of magicdance_b200.train, so
+loss.backward() runs the backward kernels with activation checkpointing where the networks' use_checkpoint
+asks for it; otherwise the inference engine.  There is no CPU path: a CPU model refuses to train.
 """
 from __future__ import annotations
 
@@ -182,11 +184,8 @@ class LatentDiffusionReferenceOnly(DDPM):
         return self.p_losses(x, c, t, *args, **kwargs)
 
     def p_losses(self, x_start, cond, t, noise=None):
-        """ddpm.py:2165-2212 — same loss and loss_dict; forward value only (no backward kernels yet)."""
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError(
-                "magicdance_b200 round 1 implements the forward (inference) kernels only; wrap the call in "
-                "torch.no_grad() to evaluate the loss, or use the reference modules for training")
+        """ddpm.py:2165-2212 — same loss and loss_dict.  Under grad mode with trainable parameters, apply_model runs
+        the differentiable forward and loss.backward() the backward kernels; otherwise the inference engine."""
         noise = torch.randn_like(x_start) if noise is None else noise
         ref = None
         if cond.get("image_control") is not None:

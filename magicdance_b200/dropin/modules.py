@@ -230,16 +230,24 @@ class UNetModel(nn.Module):
             self.middle_block_out = TimestepEmbedSequential(conv_nd(dims, mid[-1][3], mid[-1][3], 1, padding=0))
         _reset(self)
         self._packed = None
+        self._packed_params, self._packed_key = [], ()
         self.register_load_state_dict_post_hook(lambda mod, keys: mod.invalidate())
 
     # ---- engine plumbing ---------------------------------------------------------------------------
     def invalidate(self):
-        """Drop the repacked fp16 weights (call after any parameter update)."""
+        """Drop the repacked fp16 weights.  packed() notices in-place updates of the parameters by their version
+        counters; an update that bypasses them (`p.data.copy_`, an in-place collective) needs this call."""
         self._packed = None
 
     def packed(self, device=None) -> PackedNet:
+        """The inference packing of the current weights: the same object for as long as no parameter changes (so
+        that captured graphs stay valid), rebuilt after an optimizer step or a load.  The check reads the version
+        counters of the parameter list taken at packing time (walking the module tree costs milliseconds)."""
         dev = torch.device(device) if device is not None else next(self.parameters()).device
         ops.require_cuda(dev)
-        if self._packed is None or self._packed.device != dev:
+        if (self._packed is None or self._packed.device != dev
+                or tuple(p._version for p in self._packed_params) != self._packed_key):
+            self._packed_params = list(self.parameters())
+            self._packed_key = tuple(p._version for p in self._packed_params)
             self._packed = PackedNet(self.state_dict(), "", self.cfg, self._kind, dev)
         return self._packed

@@ -1062,3 +1062,21 @@ class NhwcToNchw(torch.autograd.Function):
 def nhwc_to_nchw(x, *, batch, c, h, w):
     """Differentiable nhwc_f16_to_nchw_f32() (NhwcToNchw): NHWC fp16 [B*H*W, C] -> NCHW fp32."""
     return NhwcToNchw.apply(x, batch, c, h, w)
+
+
+class Add(torch.autograd.Function):
+    """add() of two same-shaped fp16 tensors as an autograd op (the pose residuals onto the UNet's skips); both
+    gradients are dy."""
+
+    @staticmethod
+    def forward(ctx, a, b, batch):
+        return add(a, b, batch=batch)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return dy, dy, None
+
+
+def add_ad(a, b, *, batch):
+    """Differentiable add() (Add): a + b, fp16, contiguous, same shape (one b per batch element)."""
+    return Add.apply(a, b, batch)
