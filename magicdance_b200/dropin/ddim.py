@@ -1,7 +1,9 @@
 """Drop-in for DDIMSampler_ReferenceOnly (model_lib/ControlNet/ldm/models/diffusion/ddim.py:346-730):
 same constructor, make_schedule / sample / ddim_sampling / p_sample_ddim signatures and return values,
-for the configuration the MagicPose scripts drive (test_tiktok.py:261-268): eps-prediction, DDIM,
-classifier-free guidance through the 'controlnet is more important' branch (ddim.py:598-605).
+for the configuration the MagicPose scripts drive (test_tiktok.py:261-268, and the sample logging of
+train_tiktok.py:437-444 for both training stages): eps-prediction, DDIM, classifier-free guidance through the
+'controlnet is more important' branch (ddim.py:598-605).  A stage-1 model (ControlLDMReferenceOnly) has no pose
+ControlNet: the same step runs without hint features and pose residuals.
 
 Host code only: the step itself (pose ControlNet, paired conditional/unconditional UNet, fused
 CFG + DDIM update) runs on the sm_90a kernels via magicdance_b200.pipeline.DenoisePipeline, which also
@@ -125,7 +127,7 @@ class DDIMSampler_ReferenceOnly(object):
                 and uc.get("image_control") is None and scale != 1.0 and not c.get("overlap_sampling")
                 and not np.any(self.ddim_sigmas) and img.is_cuda):
             return None
-        ref, ctx, pose_map = _one(c["image_control"]), _one(c["c_crossattn"]), _one(c["c_concat"])
+        ref, ctx = _one(c["image_control"]), _one(c["c_crossattn"])
         if not (self._rows_identical(ref) and self._rows_identical(ctx)):
             return None  # one reference image and one prompt per batch only (the scripts repeat them per sample)
         pipe = self._pipeline(scale)
@@ -165,7 +167,9 @@ class DDIMSampler_ReferenceOnly(object):
                 group=group, chunk=gd.bank_chunk, storage=ent["storage"])
             ent["ref"] = ref_dev.clone()
         bank = ent["bank"]
-        gd.hint.copy_(pipe.hint(pose_map.to(pipe.device), frame_key=tensor_key(pose_map), keep_alive=pose_map))
+        if gd.has_pose:  # (a stage-1 model has no pose ControlNet and ignores c_concat)
+            pose_map = _one(c["c_concat"])
+            gd.hint.copy_(pipe.hint(pose_map.to(pipe.device), frame_key=tensor_key(pose_map), keep_alive=pose_map))
         gd.x.copy_(img.to(device=pipe.device, dtype=torch.float32))
         for i in range(total):
             index = total - i - 1
@@ -192,7 +196,9 @@ class DDIMSampler_ReferenceOnly(object):
         ref_n = ref if c["wonoise"] else self.model.q_sample(ref, t.to(dev))
         pair = lambda k: torch.cat([_one(uc[k]).to(dev), _one(c[k]).to(dev)])
         x = x.to(device=dev, dtype=torch.float32).contiguous()
-        cond_in = {"c_concat": [pair("c_concat")], "c_crossattn": [pair("c_crossattn")]}
+        cond_in = {"c_crossattn": [pair("c_crossattn")]}
+        if pipe.engine.pose is not None:  # a stage-1 model has no pose ControlNet and ignores c_concat
+            cond_in["c_concat"] = [pair("c_concat")]
         eps = self.model.apply_model(torch.cat([x, x]), torch.cat([t, t]).to(dev), cond_in, torch.cat([ref_n, ref_n]))
         e_u, e_c = eps.chunk(2)
         noise = torch.randn_like(x) if float(self.ddim_sigmas[index]) != 0.0 else None
@@ -238,7 +244,7 @@ class DDIMSampler_ReferenceOnly(object):
         pipe = self._pipeline(unconditional_guidance_scale)
         dev = pipe.device
         x = x.to(device=dev, dtype=torch.float32)
-        ref, ctx, pose_map = _one(c["image_control"]), _one(c["c_crossattn"]), _one(c["c_concat"])
+        ref, ctx = _one(c["image_control"]), _one(c["c_crossattn"])
         # the clean reference latent feeds the appearance net (ddim.py:532-533): the bank depends on (reference, t)
         # only.  One reference for the whole batch (the scripts repeat it per sample) is computed once and broadcast
         # in-kernel; the result is cached per timestep for the next frames.
@@ -247,7 +253,10 @@ class DDIMSampler_ReferenceOnly(object):
         else:  # per-sample references, or a noised one (ddim.py:535), which depends on fresh noise: not cached
             ref_in = ref if c["wonoise"] else self.model.q_sample(ref, t.to(ref.device))
             bank_kv = pipe.engine.bank_kv(ref_in, pipe.t_dev[index].expand(ref.shape[0]).contiguous(), ctx)
-        hint = pipe.hint(pose_map.to(dev), frame_key=tensor_key(pose_map), keep_alive=pose_map)
+        hint = None
+        if pipe.engine.pose is not None:  # a stage-1 model has no pose ControlNet and ignores c_concat
+            pose_map = _one(c["c_concat"])
+            hint = pipe.hint(pose_map.to(dev), frame_key=tensor_key(pose_map), keep_alive=pose_map)
         noise = None
         if float(self.ddim_sigmas[index]) != 0.0:
             noise = torch.randn_like(x)

@@ -311,7 +311,8 @@ class _BankComplete(Exception):
 
 
 class DenoiseEngine:
-    """Runs the three networks of ControlLDMReferenceOnlyPose on one GPU."""
+    """Runs the three networks of ControlLDMReferenceOnlyPose on one GPU (or, built by from_packed without a pose
+    ControlNet, the two of the stage-1 ControlLDMReferenceOnly)."""
 
     def __init__(self, state_dict, cfg: NetConfig | None = None, device="cuda"):
         ops.ensure_device()
@@ -640,17 +641,19 @@ class DenoiseEngine:
                     bank_kv=None, return_parts=False):
         """ControlLDMReferenceOnlyPose.apply_model (cldm.py:1099-1117).  Unlike the reference, the
         unconditional call does not run the pose ControlNet whose output it would discard
-        (cldm.py:1112-1114 vs 70-84)."""
+        (cldm.py:1112-1114 vs 70-84).  An engine without a pose ControlNet (self.pose None) is the stage-1
+        ControlLDMReferenceOnly.apply_model (cldm.py:1067-1077): pose_map is ignored and no residuals are added."""
         t = t.to(device=self.device, dtype=torch.int64)
-        bank = None
+        bank, pose = None, None
         if not uc:
             if bank_kv is None and reference_image_noisy is not None:
                 rb = reference_image_noisy.shape[0]
                 bank = self.appearance_write(reference_image_noisy, t[:rb], context[:rb])
                 bank_kv = self.project_bank(bank, rb)
-            if hint_feat is None:
-                hint_feat = self.hint_features(pose_map)
-            pose = self.controlnet(x_noisy, hint_feat, t, context)
+            if self.pose is not None:
+                if hint_feat is None:
+                    hint_feat = self.hint_features(pose_map)
+                pose = self.controlnet(x_noisy, hint_feat, t, context)
         else:
             pose, bank_kv = None, None
         taps = [] if return_parts else None

@@ -115,10 +115,11 @@ class DenoisePipeline:
     # ---- one DDIM step ---------------------------------------------------------------------------
     def step(self, x, index, context, hint_feat, bank_kv, noise=None):
         """p_sample_ddim (ddim.py:518-645): eps_c = apply_model(x,t,c,ref), eps_u = apply_model(x,t,c,None,uc),
-        CFG combine, DDIM update.  x: fp32 NCHW on the device.  Returns (x_prev, pred_x0, eps_c, eps_u)."""
+        CFG combine, DDIM update.  x: fp32 NCHW on the device.  Returns (x_prev, pred_x0, eps_c, eps_u).
+        Without a pose ControlNet (stage 1) hint_feat is not read and no residuals are added."""
         eng = self.engine
         t = self.t_dev[index:index + 1]  # one timestep for the whole batch (a view: no kernel)
-        pose = eng.controlnet(x, hint_feat, t, context)
+        pose = None if eng.pose is None else eng.controlnet(x, hint_feat, t, context)
         eps_c, eps_u = eng.unet_forward(x, t, context, bank_kv=bank_kv, pose=pose, cfg_pair=True)
         x_prev, pred_x0 = ops.cfg_ddim_update(x.contiguous(), eps_c.contiguous(), eps_u.contiguous(), self.coef[index],
                                               noise=noise)
@@ -130,7 +131,7 @@ class DenoisePipeline:
         x = x_T.to(device=self.device, dtype=torch.float32).contiguous()
         context = context.to(self.device)
         ref_latent = ref_latent.to(self.device)
-        hint_feat = self.hint(pose_map.to(self.device), frame_key)
+        hint_feat = None if self.engine.pose is None else self.hint(pose_map.to(self.device), frame_key)
         pred_x0 = x
         for i in range(self.ddim_steps):
             index = self.ddim_steps - 1 - i
@@ -182,7 +183,10 @@ class GraphedDenoiser:
         self.t_cur = torch.zeros((1,), dtype=torch.int64, device=dev)
         self.t_vec = torch.zeros((bank_chunk,), dtype=torch.int64, device=dev)
         self.coef_cur = torch.zeros((8,), dtype=torch.float32, device=dev)
-        self.hint = torch.zeros((batch * h * w, eng.cfg.model_channels), dtype=torch.float16, device=dev)
+        self.has_pose = eng.pose is not None  # stage 1 (ControlLDMReferenceOnly) has no pose ControlNet
+        self.hint = None
+        if self.has_pose:
+            self.hint = torch.zeros((batch * h * w, eng.cfg.model_channels), dtype=torch.float16, device=dev)
         geo = eng.attn_geometry(h, w)
         self.tokens = [n for n, _ in geo]
         self.layout = parallel.BankLayout([(n, c) for n, c in geo])
@@ -191,18 +195,22 @@ class GraphedDenoiser:
         # timestep path hoisted out of the step: embedding -> time_embed MLP -> all emb_layers depend on t only, so the
         # tables for every ddim index are computed once (capture()) and a step copies its two rows into these buffers
         self.emb_unet = torch.zeros((1, eng.unet.emb_total), dtype=torch.float32, device=dev)
-        self.emb_pose = torch.zeros((1, eng.pose.emb_total), dtype=torch.float32, device=dev)
+        self.emb_pose = self.side = None
+        if self.has_pose:
+            self.emb_pose = torch.zeros((1, eng.pose.emb_total), dtype=torch.float32, device=dev)
+            self.side = torch.cuda.Stream(device=dev)  # the pose ControlNet's stream (joins the UNet at the middle block)
         self.emb_tab_unet = self.emb_tab_pose = None
         self.g_step = self.g_bank = None
         self.replayed_launches = 0
-        self.side = torch.cuda.Stream(device=dev)  # the pose ControlNet's stream (joins the UNet at the middle block)
         # auxiliary streams for independent branches inside a block (engine._fork): lane 0 (UNet pass) -> lane 2,
         # lane 1 (ControlNet pass on the side stream) -> lane 3
         # (kept on THIS object and handed to the engine only for the duration of _step_body: eager calls through the
         # same engine must not inherit the fork/join path and its scratch lanes)
         self.aux_streams = None
         if batch <= 2:
-            self.aux_streams = {0: (torch.cuda.Stream(device=dev), 2), 1: (torch.cuda.Stream(device=dev), 3)}
+            self.aux_streams = {0: (torch.cuda.Stream(device=dev), 2)}
+            if self.has_pose:
+                self.aux_streams[1] = (torch.cuda.Stream(device=dev), 3)
 
     # the two bodies, written against the static buffers only
     def _step_body(self):
@@ -220,6 +228,11 @@ class GraphedDenoiser:
     def _step_body_inner(self, eng, b):
         t = self.t_cur  # one timestep for the whole batch
         bank_kv = self.layout.views(self.bank_cur, self.tokens, 1)
+        if not self.has_pose:
+            eps_c, eps_u = eng.unet_forward(self.x, t, self.ctx, bank_kv=bank_kv, cfg_pair=True, emb_all=self.emb_unet)
+            ops.cfg_ddim_update(self.x, eps_c, eps_u, self.coef_cur, x_prev=self.x_prev, pred_x0=self.pred_x0,
+                                update_x=True)
+            return
         main = torch.cuda.current_stream()
         self.side.wait_stream(main)
         with torch.cuda.stream(self.side), ops.workspace_lane(1):
@@ -240,9 +253,11 @@ class GraphedDenoiser:
         with torch.cuda.stream(s):
             eng, td = self.eng, self.pipe.t_dev
             self.emb_tab_unet = torch.cat([eng.time_bias(eng.unet, td[i:i + 1]) for i in range(td.shape[0])], 0)
-            self.emb_tab_pose = torch.cat([eng.time_bias(eng.pose, td[i:i + 1]) for i in range(td.shape[0])], 0)
+            if self.has_pose:
+                self.emb_tab_pose = torch.cat([eng.time_bias(eng.pose, td[i:i + 1]) for i in range(td.shape[0])], 0)
             self.emb_unet.copy_(self.emb_tab_unet[-1:])
-            self.emb_pose.copy_(self.emb_tab_pose[-1:])
+            if self.has_pose:
+                self.emb_pose.copy_(self.emb_tab_pose[-1:])
             for _ in range(2):
                 self._bank_body()
                 self._step_body()
@@ -281,7 +296,8 @@ class GraphedDenoiser:
         self.t_cur.copy_(self.pipe.t_dev[index:index + 1])
         self.coef_cur.copy_(self.pipe.coef[index])
         self.emb_unet.copy_(self.emb_tab_unet[index:index + 1])
-        self.emb_pose.copy_(self.emb_tab_pose[index:index + 1])
+        if self.has_pose:
+            self.emb_pose.copy_(self.emb_tab_pose[index:index + 1])
         self.bank_cur.copy_(bank_flat)
         self.g_step.replay()
         self.replayed_launches += self.step_launches

@@ -1,5 +1,6 @@
 """Differentiable forward of the three networks on the sm_90a kernels: the training counterpart of
-engine.DenoiseEngine.apply_model (uc=False) for ControlLDMReferenceOnlyPose.p_losses (ddpm.py:2165-2212).
+engine.DenoiseEngine.apply_model (uc=False) for ControlLDMReferenceOnlyPose.p_losses (ddpm.py:2165-2212), and of the
+two networks of the stage-1 ControlLDMReferenceOnly (no pose ControlNet).
 
 It walks the same engine.block_plan as the inference engine, but every layer is one of the autograd ops of
 magicdance_b200.ops (tc_gemm, two_source_attention, group_norm, layer_norm, geglu, direct_conv3x3, skinny_linear_ad,
@@ -430,19 +431,22 @@ def controlnet(net: TrainNet, x: Act, hint, t, text):
 
 
 def unet(net: TrainNet, x: Act, t, text, bank, pose):
-    """ControlledUnetModelAttnPose.forward (cldm.py:59-112) in 'read' mode: NHWC fp16 [B*H*W, out_channels]"""
+    """ControlledUnetModelAttnPose.forward (cldm.py:59-112) in 'read' mode: NHWC fp16 [B*H*W, out_channels].
+    pose None: ControlledUnetModelAttn.forward (cldm.py:115-161), the stage-1 UNet without residual adds."""
     emb_all = _time_bias(net, t, x.b)
     st = {"mode": "read", "attn_i": 0, "bank": bank}
-    pose = list(pose)
+    pose = None if pose is None else list(pose)
     hs = []
     for i, blk in enumerate(net.inp):
         x = _run_block(net, f"input_blocks.{i}.", blk, x, None, emb_all, text, st)
         hs.append(x)
     x = _run_block(net, "middle_block.", net.mid, x, None, emb_all, text, st)
-    x = Act(ops.add_ad(x.data, pose.pop(), batch=x.b), x.b, x.h, x.w)
+    if pose is not None:
+        x = Act(ops.add_ad(x.data, pose.pop(), batch=x.b), x.b, x.h, x.w)
     for i, blk in enumerate(net.out):
         s = hs.pop()
-        s = Act(ops.add_ad(s.data, pose.pop(), batch=s.b), s.b, s.h, s.w)
+        if pose is not None:
+            s = Act(ops.add_ad(s.data, pose.pop(), batch=s.b), s.b, s.h, s.w)
         x = _run_block(net, f"output_blocks.{i}.", blk, x, s, emb_all, text, st)
     hn = ops.group_norm(x.data, *net.out_gn, batch=x.b, hw=x.hw, eps=1e-5, silu=True)
     return _conv3x3(Act(hn, x.b, x.h, x.w), net.out_w, net.cfg.out_channels, bias=net.out_b)
@@ -452,8 +456,9 @@ def apply_model(unet_module, appearance_module, pose_module, x_noisy, t, context
     """ControlLDMReferenceOnlyPose.apply_model (cldm.py:1099-1117, uc=False) as a differentiable function of every
     parameter of the three drop-in networks that requires grad, and of x_noisy (and context) when they do.
     Returns eps as NCHW fp32.  reference_latent: the appearance net's input (the clean latent with wonoise), one per
-    sample, or None (no bank)."""
-    modules = (unet_module, appearance_module, pose_module)
+    sample, or None (no bank).  pose_module None: the stage-1 ControlLDMReferenceOnly.apply_model (cldm.py:1067-1077),
+    with no hint path, no pose ControlNet and no residual adds; pose_map is not read."""
+    modules = tuple(m for m in (unet_module, appearance_module, pose_module) if m is not None)
     try:
         for dev in {x_noisy.device} | {p.device for m in modules for p in m.parameters()}:
             ops.require_cuda(dev)
@@ -469,7 +474,8 @@ def apply_model(unet_module, appearance_module, pose_module, x_noisy, t, context
     gs = GradScale()
     with torch.autocast("cuda", enabled=False):
         # fp16 copies of the trained weights: once per forward, outside every checkpointed region
-        un, app, pose = TrainNet(unet_module, gs), TrainNet(appearance_module, gs), TrainNet(pose_module, gs)
+        un, app = TrainNet(unet_module, gs), TrainNet(appearance_module, gs)
+        pose = None if pose_module is None else TrainNet(pose_module, gs)
         t = t.to(device=dev, dtype=torch.int64).reshape(-1)
         if t.shape[0] == 1 and b > 1:
             t = t.expand(b).contiguous()
@@ -482,8 +488,10 @@ def apply_model(unet_module, appearance_module, pose_module, x_noisy, t, context
         if reference_latent is not None:
             ref = _input(reference_latent.to(device=dev, dtype=torch.float32), gs)
             bank = appearance_write(app, Act(ops.nchw_to_nhwc(ref), b, h, w), t, text)
-        hint = hint_features(pose, _input(pose_map.to(device=dev, dtype=torch.float32), gs).contiguous())
-        residuals = controlnet(pose, x16, hint, t, text)
+        residuals = None
+        if pose is not None:
+            hint = hint_features(pose, _input(pose_map.to(device=dev, dtype=torch.float32), gs).contiguous())
+            residuals = controlnet(pose, x16, hint, t, text)
         y = unet(un, x16, t, text, bank, residuals)
         eps = ops.nhwc_to_nchw(y.data, batch=b, c=un.cfg.out_channels, h=h, w=w)
         return _ScaleOut.apply(eps, gs)

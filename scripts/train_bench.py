@@ -12,7 +12,11 @@ ms/step and peak allocated memory per mode, and algorithmic TFLOP/s against the 
 oracle/count_training_flops.py counted on the reference (stage-2 freeze, with the checkpoint recompute).  Writes nothing
 to the tree.
 
-    python scripts/train_bench.py [--batch 4] [--latent 64] [--steps 5] [--warmup 2] [--modes ckpt,plain]
+With --stage 1 it measures stage-1 appearance-control pre-training instead (models/cldm_v15_reference_only.yaml,
+scripts/appearance_control_pretraining.sh: ControlLDMReferenceOnly, the appearance net trained, the same UNet freeze, its
+time_embed reached by the gradient); no reference FLOP count is taken for it.
+
+    python scripts/train_bench.py [--stage 2] [--batch 4] [--latent 64] [--steps 5] [--warmup 2] [--modes ckpt,plain]
 """
 from __future__ import annotations
 
@@ -44,13 +48,18 @@ def gpu_info():
     return name, limit
 
 
-def build_model():
+def build_model(stage=2):
     import torch
     from magicdance_b200 import synth
     from model_lib.ControlNet.cldm.model import create_model
-    model = create_model(os.path.join(REPO, "model_lib", "ControlNet", "models", "cldm_v15_reference_only_pose.yaml"))
-    sd = synth.synth_state_dict(seed=0)
+    yaml = "cldm_v15_reference_only_pose.yaml" if stage == 2 else "cldm_v15_reference_only.yaml"
+    model = create_model(os.path.join(REPO, "model_lib", "ControlNet", "models", yaml))
     own = model.state_dict()
+    if stage == 2:
+        sd = synth.synth_state_dict(seed=0)
+    else:  # the stage-1 layout: synthesised per key of the model's own state dict
+        sd = synth.synth_state_dict({k: list(v.shape) for k, v in own.items()
+                                     if k not in synth.SCHEDULE_KEYS and not k.startswith("first_stage_model.")}, seed=0)
     sd.update({k: own[k] for k in own if k not in sd})
     model.load_state_dict(sd, strict=True)
     dm = model.model.diffusion_model
@@ -62,7 +71,7 @@ def build_model():
 def run(model, batch, latent, steps, warmup, checkpointing):
     import torch
     from magicdance_b200 import synth
-    for net in (model.model.diffusion_model, model.appearance_control_model, model.pose_control_model):
+    for net in (n for n in model._nets() if n is not None):
         net.use_checkpoint = checkpointing
     opt = torch.optim.AdamW([p for p in model.parameters() if p.requires_grad], lr=1e-5)
     inp = {k: v.cuda() for k, v in synth.synth_inputs(batch, latent, seed=0, shared_reference=False).items()}
@@ -93,6 +102,8 @@ def run(model, batch, latent, steps, warmup, checkpointing):
            "peak_allocated_gib": torch.cuda.max_memory_allocated() / 2 ** 30,
            "algorithmic_tflops_vs_reference_count": REFERENCE_GF_PER_SAMPLE * batch / ms,
            "finite": bool(torch.isfinite(loss))}
+    if model._nets()[2] is None:  # the reference FLOP count is stage 2's
+        del res["algorithmic_tflops_vs_reference_count"]
     del opt
     model.zero_grad(set_to_none=True)
     torch.cuda.empty_cache()
@@ -101,6 +112,8 @@ def run(model, batch, latent, steps, warmup, checkpointing):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--stage", type=int, default=2, choices=(1, 2),
+                    help="2: appearance-disentangled pose control; 1: appearance-control pre-training")
     ap.add_argument("--batch", type=int, default=4)
     ap.add_argument("--latent", type=int, default=64)
     ap.add_argument("--steps", type=int, default=5)
@@ -110,10 +123,15 @@ def main():
     import torch
     assert torch.cuda.is_available(), "needs an sm_90 GPU"
     name, limit = gpu_info()
-    model = build_model()
-    out = {"metric": "training samples/s (BASELINE config 5, stage 2, one GPU)", "device": name, "power_limit_w": limit,
-           "batch": args.batch, "latent": args.latent, "steps": args.steps, "warmup": args.warmup,
-           "reference_gf_per_sample": REFERENCE_GF_PER_SAMPLE}
+    model = build_model(args.stage)
+    if args.stage == 2:
+        out = {"metric": "training samples/s (BASELINE config 5, stage 2, one GPU)", "device": name,
+               "power_limit_w": limit, "batch": args.batch, "latent": args.latent, "steps": args.steps,
+               "warmup": args.warmup, "reference_gf_per_sample": REFERENCE_GF_PER_SAMPLE}
+    else:
+        out = {"metric": "training samples/s (stage 1 appearance-control pre-training, one GPU)", "device": name,
+               "power_limit_w": limit, "batch": args.batch, "latent": args.latent, "steps": args.steps,
+               "warmup": args.warmup}
     for mode in args.modes.split(","):
         try:
             out[mode] = run(model, args.batch, args.latent, args.steps, args.warmup, checkpointing=mode == "ckpt")
