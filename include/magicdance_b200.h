@@ -141,6 +141,25 @@ int mdb_gemm_bwd_f16(const mdb_gemm_bwd_desc* desc, mdb_stream_t stream);
 int64_t mdb_gemm_bwd_ws_floats(const mdb_gemm_bwd_desc* desc);
 
 /* ------------------------------------------------------------------------------------------------
+ * 3x3 pad-1 convolution (conv_nd of ResBlock / Upsample / Downsample, openaimodel.py:127,175,225,249-252) at ANY
+ * latent size, forward and backward, on the same wgmma kernels: the activation tiles come from TMA im2col-mode loads,
+ * which walk 128 consecutive output pixels across row and image boundaries and zero-fill the halo, instead of the 4-D
+ * boxes of mdb_gemm_f16's conv mode (which need the pixels of a tile to form a box, e.g. 16x16 ... 128x128 latents).
+ * At sizes both take, the two give bit-equal results.  Same descriptors as mdb_gemm_f16 / mdb_gemm_bwd_f16 with:
+ *   conv     1 | 2: the stride (required);  nb, h, w, c: the input, c % 64 == 0;  k = 9c;  m = nb * ho * wo
+ *   a, lda   NHWC fp16 input, lda = the pixel stride in elements (0: the channel count)
+ *   a2, lda2 optional second source (a fused torch.cat along channels): channels [0, k1) of every pixel come from a,
+ *            [k1, c) from a2; k1 a multiple of 64.  Ignored (k1 = c) when a2 == NULL
+ *   epilogue MDB_EPI_NONE, ln_u NULL; bias / per-batch bias / residual / splits / splitk_ws as in mdb_gemm_f16
+ * The backward's gradients are those of mdb_gemm_bwd_f16 (da: [nb*h*w][k1], da2: [nb*h*w][c - k1]); dA at stride 2
+ * goes through the fp32 column buffer and gather kernel (single source only), everything else through im2col loads.
+ * ---------------------------------------------------------------------------------------------- */
+int mdb_conv3x3_igemm_f16(const mdb_gemm_desc* desc, mdb_stream_t stream);
+int mdb_conv3x3_igemm_bwd_f16(const mdb_gemm_bwd_desc* desc, mdb_stream_t stream);
+/* workspace floats mdb_conv3x3_igemm_bwd_f16 needs; negative MDB_ERR_* for a descriptor it rejects */
+int64_t mdb_conv3x3_igemm_bwd_ws_floats(const mdb_gemm_bwd_desc* desc);
+
+/* ------------------------------------------------------------------------------------------------
  * Fused attention, FlashAttention-style tile loop on wgmma, with TWO key/value sources whose
  * keys are concatenated in-kernel:  out = softmax([Q K0^T | Q K1^T] * scale) [V0 ; V1].
  * Replaces CrossAttention._forward (attention.py:168-199) / MemoryEfficientCrossAttention

@@ -121,6 +121,9 @@ SIGNATURES = {
     "mdb_gemm_f16": (c_int32, [C.POINTER(GemmDesc), c_void_p]),
     "mdb_gemm_bwd_f16": (c_int32, [C.POINTER(GemmBwdDesc), c_void_p]),
     "mdb_gemm_bwd_ws_floats": (c_int64, [C.POINTER(GemmBwdDesc)]),
+    "mdb_conv3x3_igemm_f16": (c_int32, [C.POINTER(GemmDesc), c_void_p]),
+    "mdb_conv3x3_igemm_bwd_f16": (c_int32, [C.POINTER(GemmBwdDesc), c_void_p]),
+    "mdb_conv3x3_igemm_bwd_ws_floats": (c_int64, [C.POINTER(GemmBwdDesc)]),
     "mdb_attention_f16": (c_int32, [C.POINTER(AttnDesc), c_void_p]),
     "mdb_attention_lse_f16": (c_int32, [C.POINTER(AttnDesc), c_void_p, c_void_p]),
     "mdb_attention_bwd_f16": (c_int32, [C.POINTER(AttnBwdDesc), c_void_p]),

@@ -66,6 +66,13 @@ int tmap_vt(CUtensorMap* out, const void* base, int n, int nb, long long ldvb, i
 // pixel along w and h (TMA element strides)
 int tmap_nhwc(CUtensorMap* out, const void* base, int c, int w, int h, int nb, long long ld, const uint32_t box[4],
               int cs);
+// The same NHWC images as an im2col-mode map for a 3x3 pad-1 window: one load walks `pixels` consecutive window
+// positions (output pixels) across row and image boundaries, 64 channels each, into the [pixels][64] 128B-swizzled
+// tile a tiled box of `pixels` rows gives.  The load's coordinates are the window's top-left input pixel
+// (cs * x - 1, cs * y - 1) of the first output pixel; its im2col offsets (0..2 along w and h) pick the tap; pixels
+// outside the image are zero-filled.  cs = 2 steps the window by two input pixels (TMA element strides).
+int tmap_nhwc_im2col(CUtensorMap* out, const void* base, int c, int w, int h, int nb, long long ld, int pixels,
+                     int cs);
 
 // The 4-D TMA box {64 channels, x, y, images} that covers `rows` consecutive output pixels of a 3x3 conv with ho x wo
 // output pixels per image, reading every cs-th input pixel.  `fwd` selects the forward kernel's rule for rows at
@@ -238,6 +245,18 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+// im2col-mode load of a tmap_nhwc_im2col map: coordinates (channel, w, h, image) of the first window's corner, offsets
+// (ow, oh) of the tap inside the window
+__device__ __forceinline__ void tma_load_im2col_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                   int c2, int c3, int ow, int oh) {
+  const uint16_t w16 = static_cast<uint16_t>(ow), h16 = static_cast<uint16_t>(oh);
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3),
+        "h"(w16), "h"(h16)
       : "memory");
 }
 

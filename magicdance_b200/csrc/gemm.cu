@@ -117,9 +117,12 @@ __device__ __forceinline__ void epi_store_chunk(const GemmKParams& p, long long 
   }
 }
 
-template <int BN, bool GEGLU, int kStages>
-__global__ void __launch_bounds__(kWsThreads, (GemmSmem<BN, kStages>::kCtasPerSm))
-    gemm_tc_kernel(const __grid_constant__ GemmKParams p) {
+// IM2COL: the 3x3 conv's A tiles come from TMA im2col loads (tmap_nhwc_im2col), which walk 128 consecutive output
+// pixels across row and image boundaries: any latent size, one or two sources split along the channels (k1_chunks of
+// the chunks_per_tap chunks of a tap from tmA, the rest from tmA2).  The tiles are the ones the 4-D boxes give at sizes
+// that tile, so everything after the producer is shared.
+template <int BN, bool GEGLU, int kStages, bool IM2COL>
+__device__ __forceinline__ void gemm_tc_body(const GemmKParams& p) {
   using S = GemmSmem<BN, kStages>;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kStages];
@@ -144,6 +147,7 @@ __global__ void __launch_bounds__(kWsThreads, (GemmSmem<BN, kStages>::kCtasPerSm
   pdl_launch_dependents();
   if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&p.tmA);
+    if constexpr (IM2COL) tma_prefetch_desc(&p.tmA2);
     tma_prefetch_desc(&p.tmB);
     ring_init<kStages>(full_bar, empty_bar, 1);
     fence_barrier_init();
@@ -164,7 +168,11 @@ __global__ void __launch_bounds__(kWsThreads, (GemmSmem<BN, kStages>::kCtasPerSm
     if (lane == 0 && n_iter > 0) {
       // conv geometry of this M tile
       int b0 = 0, y0 = 0, x0 = 0;
-      if (p.conv) {
+      if constexpr (IM2COL) {  // the first output pixel of this M tile; the tile may run on into later rows and images
+        b0 = m0 / p.hw;
+        y0 = (m0 - b0 * p.hw) / p.w;
+        x0 = (m0 - b0 * p.hw) - y0 * p.w;
+      } else if (p.conv) {
         b0 = m0 / p.hw;
         y0 = (p.hw >= kBM) ? (m0 % p.hw) / p.w : 0;
         x0 = (p.hw >= kBM) ? (m0 % p.hw) % p.w : 0;  // != 0 only for rows wider than the 128-pixel tile
@@ -175,7 +183,14 @@ __global__ void __launch_bounds__(kWsThreads, (GemmSmem<BN, kStages>::kCtasPerSm
         uint8_t* sb = sa + S::kABytes;
         const int kc = kc_begin + it;
         mbar_expect_tx(&full_bar[s], S::kStageBytes);
-        if (p.conv) {
+        if constexpr (IM2COL) {
+          const int tap = kc / p.chunks_per_tap;
+          const int cc = kc - tap * p.chunks_per_tap;
+          const int kh = tap / 3, kw = tap - kh * 3;
+          const int xs = p.cs * x0 - 1, ys = p.cs * y0 - 1;  // the first window's corner; the tap is the offset
+          if (cc < p.k1_chunks) tma_load_im2col_4d(sa, &p.tmA, &full_bar[s], cc * kBK, xs, ys, b0, kw, kh);
+          else tma_load_im2col_4d(sa, &p.tmA2, &full_bar[s], (cc - p.k1_chunks) * kBK, xs, ys, b0, kw, kh);
+        } else if (p.conv) {
           const int tap = kc / p.chunks_per_tap;
           const int cc = kc - tap * p.chunks_per_tap;
           const int kh = tap / 3, kw = tap - kh * 3;
@@ -442,7 +457,18 @@ __global__ void __launch_bounds__(kWsThreads, (GemmSmem<BN, kStages>::kCtasPerSm
       cluster_sync_all();  // nobody leaves while a partner may still read its shared memory
     }
   }
+}
 
+template <int BN, bool GEGLU, int kStages>
+__global__ void __launch_bounds__(kWsThreads, (GemmSmem<BN, kStages>::kCtasPerSm))
+    gemm_tc_kernel(const __grid_constant__ GemmKParams p) {
+  gemm_tc_body<BN, GEGLU, kStages, false>(p);
+}
+
+template <int BN, int kStages>
+__global__ void __launch_bounds__(kWsThreads, (GemmSmem<BN, kStages>::kCtasPerSm))
+    gemm_igemm_kernel(const __grid_constant__ GemmKParams p) {
+  gemm_tc_body<BN, false, kStages, true>(p);
 }
 
 // split-K second pass: sum of the fp32 partial slabs ws[splits][M][N] -> bias/residual -> fp16 D
@@ -519,10 +545,9 @@ static int g_pair_min_tiles = 128;  // smallest grid, in 128-row tile equivalent
 static int g_bn80_below = 100;      // N % 160 == 0 layers with fewer 160-wide CTAs than this use 80-wide tiles
 constexpr int kLongKChunks = 64;    // ... unless K >= 4096 (automatic split-K): then 160-wide tiles and split K
 
-template <int BN, bool GEGLU, int STAGES>
-static int launch_gemm(const GemmKParams& kp, dim3 grid, cudaStream_t st) {
+template <auto kern, int BN, int STAGES>
+static int launch_kernel(const GemmKParams& kp, dim3 grid, cudaStream_t st) {
   const unsigned cluster_z = kp.cluster_reduce ? static_cast<unsigned>(kp.splits) : 1u;
-  constexpr auto kern = gemm_tc_kernel<BN, GEGLU, STAGES>;
   constexpr int kSmem = GemmSmem<BN, STAGES>::kTotal;
   static_assert(kSmem <= 227 * 1024, "shared memory budget");
   if (int rc = set_max_dyn_smem<kern>(kSmem)) return rc;
@@ -530,11 +555,113 @@ static int launch_gemm(const GemmKParams& kp, dim3 grid, cudaStream_t st) {
   count_launch();
   return MDB_OK;
 }
+// IM2COL: the conv at any size (gemm_igemm_kernel, never with GEGLU), else gemm_tc_kernel
+template <int BN, bool GEGLU, int STAGES, bool IM2COL>
+static int launch_gemm(const GemmKParams& kp, dim3 grid, cudaStream_t st) {
+  if constexpr (IM2COL) {
+    static_assert(!GEGLU, "the im2col conv has no GEGLU epilogue");
+    return launch_kernel<gemm_igemm_kernel<BN, STAGES>, BN, STAGES>(kp, grid, st);
+  } else {
+    return launch_kernel<gemm_tc_kernel<BN, GEGLU, STAGES>, BN, STAGES>(kp, grid, st);
+  }
+}
 
 int get_gemm_tuning(int key) { return key == MDB_TUNE_GEMM_PAIR_MIN_TILES ? g_pair_min_tiles : g_bn80_below; }
 void set_gemm_tuning(int key, int value) {
   if (key == MDB_TUNE_GEMM_PAIR_MIN_TILES) g_pair_min_tiles = value;
   else g_bn80_below = value;
+}
+
+// tile width, split-K and kernel choice for a descriptor validated and A-mapped by the caller: the same rules for the
+// GEMM, the box-path conv and (IM2COL) the conv at any size
+template <bool IM2COL>
+static int dispatch(const char* fn, const mdb_gemm_desc* g, GemmKParams& kp, bool geglu, cudaStream_t st) {
+  int rc;
+  // ---- which kernel ----
+  // Large grids (>= g_pair_min_tiles 128-row tile equivalents, no split-K, at least two M tiles): 128 x 256 tiles
+  // (N % 256 == 0) or 128 x 160 / 128 x 128 tiles with deep rings, one CTA per SM — widest first: fewest L2 -> SM
+  // bytes per flop.
+  const int m_tiles = (g->m + kBM - 1) / kBM;
+  bool pair = g->splits <= 1 && m_tiles >= 2 && g->n % 8 == 0 && g->ln_u == nullptr;
+  int bn = 0;
+  if (pair) {
+    if (geglu) bn = (g->n % 256 == 0) ? 256 : 0;
+    else if (g->n % 256 == 0) bn = 256;
+    else if (g->n % 160 == 0) bn = 160;
+    else bn = 128;
+    // ... and enough work per launch: only a large grid AND a K loop that is not a handful of chunks pays for the
+    // single-CTA-per-SM tiles
+    const long long eq = (long long)m_tiles * ((g->n + bn - 1) / (bn ? bn : 1));
+    if (bn == 0 || eq < (long long)g_pair_min_tiles || eq * kp.k_chunks < 16ll * g_pair_min_tiles) pair = false;
+  }
+  if (pair) {
+    // bn chosen above
+  } else if (geglu) {
+    MDB_REQUIRE(g->n % 128 == 0, "%s: GEGLU needs N %% 128 == 0 (N=%d)", fn, g->n);
+    bn = 128;
+  } else if (g->n % 160 == 0) {
+    // 160-wide tiles unless that leaves most of the SMs idle; then (short K) halve the tile width, or (long K:
+    // the weight-streaming 3x3 convs of the 8x8 ... 32x32 levels at one frame) keep the wide tile and split K —
+    // see the automatic split-K below (scripts/gpu_microbench.py times the tile width x split-K choices)
+    const long long tiles160 = (long long)m_tiles * (g->n / 160) * (g->splits > 1 ? g->splits : 1);
+    const bool wide_split = g->splits == 0 && kp.k_chunks >= kLongKChunks && tiles160 * 2 <= kNumSms;
+    bn = (tiles160 < g_bn80_below && !wide_split) ? 80 : 160;
+  } else {
+    bn = 128;
+  }
+  rc = tmap_rows(&kp.tmB, g->b, g->k, g->n, g->ldb, kBK, bn);
+  if (rc) return rc;
+
+  int splits = g->splits > 1 ? g->splits : 1;
+  if (g->ln_u != nullptr) splits = 1;  // the correction is applied by the CTA that holds the whole K range
+  if (g->splits == 0 && !geglu && !pair && g->ln_u == nullptr) {
+    // automatic split-K: a power of two up to 8 (reduced inside a thread-block cluster through DSMEM) that brings
+    // the grid to about one CTA per SM while every split keeps at least 16 K chunks (below that the cluster
+    // reduction costs more than the extra CTAs gain)
+    const long long tiles = (long long)m_tiles * ((g->n + bn - 1) / bn);
+    if (tiles < 100)
+      for (int c = 8; c >= 2; c >>= 1)
+        if (tiles * c <= kNumSms && kp.k_chunks / c >= 16) {
+          splits = c;
+          break;
+        }
+  }
+  if (splits > kp.k_chunks) splits = kp.k_chunks;
+  if (geglu || pair) splits = 1;
+  kp.chunks_per_split = (kp.k_chunks + splits - 1) / splits;
+  splits = (kp.k_chunks + kp.chunks_per_split - 1) / kp.chunks_per_split;  // no empty splits
+  kp.splits = splits;
+  kp.ws = g->splitk_ws;
+  // 2, 4 or 8 splits: the partners form a thread-block cluster and reduce through DSMEM (one kernel);
+  // other counts go through the global fp32 workspace + finalize kernel.
+  kp.cluster_reduce = (!geglu && (splits == 2 || splits == 4 || splits == 8)) ? 1 : 0;
+  if (splits > 1 && !kp.cluster_reduce) {
+    MDB_REQUIRE(g->splitk_ws != nullptr, "%s: splits > 1 needs splitk_ws", fn);
+  }
+
+  dim3 grid(m_tiles, (g->n + bn - 1) / bn, splits);
+  const bool deep = (long long)grid.x * grid.y * grid.z <= kNumSms && kp.chunks_per_split >= 12;
+  if constexpr (!IM2COL) {
+    if (geglu) return pair ? launch_gemm<256, true, 4, false>(kp, grid, st) : launch_gemm<128, true, 3, false>(kp, grid, st);
+  }
+  if (pair) {
+    if (bn == 256) rc = launch_gemm<256, false, 4, IM2COL>(kp, grid, st);
+    else if (bn == 160) rc = launch_gemm<160, false, 6, IM2COL>(kp, grid, st);
+    else rc = launch_gemm<128, false, 6, IM2COL>(kp, grid, st);
+    return rc;
+  }
+  if (bn == 160) rc = deep ? launch_gemm<160, false, 6, IM2COL>(kp, grid, st) : launch_gemm<160, false, 3, IM2COL>(kp, grid, st);
+  else if (bn == 80) rc = deep ? launch_gemm<80, false, 8, IM2COL>(kp, grid, st) : launch_gemm<80, false, 3, IM2COL>(kp, grid, st);
+  else rc = deep ? launch_gemm<128, false, 6, IM2COL>(kp, grid, st) : launch_gemm<128, false, 3, IM2COL>(kp, grid, st);
+  if (rc) return rc;
+  if (splits > 1 && !kp.cluster_reduce) {
+    const long long total = ((long long)g->m * g->n + 3) / 4;
+    int blocks = (int)((total + 255) / 256);
+    if (blocks > kNumSms * 8) blocks = kNumSms * 8;
+    MDB_CHECK_CUDA(launch_pdl(splitk_finalize_kernel, dim3(blocks), dim3(256), 0, st, kp));
+    count_launch();
+  }
+  return MDB_OK;
 }
 
 }  // namespace mdb
@@ -617,87 +744,60 @@ extern "C" int mdb_gemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
     kp.k1_chunks = k1 / kBK;
   }
 
-  // ---- which kernel ----
-  // Large grids (>= g_pair_min_tiles 128-row tile equivalents, no split-K, at least two M tiles): 128 x 256 tiles
-  // (N % 256 == 0) or 128 x 160 / 128 x 128 tiles with deep rings, one CTA per SM — widest first: fewest L2 -> SM
-  // bytes per flop.
-  const int m_tiles = (g->m + kBM - 1) / kBM;
-  bool pair = g->splits <= 1 && m_tiles >= 2 && g->n % 8 == 0 && g->ln_u == nullptr;
-  int bn = 0;
-  if (pair) {
-    if (geglu) bn = (g->n % 256 == 0) ? 256 : 0;
-    else if (g->n % 256 == 0) bn = 256;
-    else if (g->n % 160 == 0) bn = 160;
-    else bn = 128;
-    // ... and enough work per launch: only a large grid AND a K loop that is not a handful of chunks pays for the
-    // single-CTA-per-SM tiles
-    const long long eq = (long long)m_tiles * ((g->n + bn - 1) / (bn ? bn : 1));
-    if (bn == 0 || eq < (long long)g_pair_min_tiles || eq * kp.k_chunks < 16ll * g_pair_min_tiles) pair = false;
-  }
-  if (pair) {
-    // bn chosen above
-  } else if (geglu) {
-    MDB_REQUIRE(g->n % 128 == 0, "mdb_gemm_f16: GEGLU needs N %% 128 == 0 (N=%d)", g->n);
-    bn = 128;
-  } else if (g->n % 160 == 0) {
-    // 160-wide tiles unless that leaves most of the SMs idle; then (short K) halve the tile width, or (long K:
-    // the weight-streaming 3x3 convs of the 8x8 ... 32x32 levels at one frame) keep the wide tile and split K —
-    // see the automatic split-K below (scripts/gpu_microbench.py times the tile width x split-K choices)
-    const long long tiles160 = (long long)m_tiles * (g->n / 160) * (g->splits > 1 ? g->splits : 1);
-    const bool wide_split = g->splits == 0 && kp.k_chunks >= kLongKChunks && tiles160 * 2 <= kNumSms;
-    bn = (tiles160 < g_bn80_below && !wide_split) ? 80 : 160;
-  } else {
-    bn = 128;
-  }
-  rc = tmap_rows(&kp.tmB, g->b, g->k, g->n, g->ldb, kBK, bn);
-  if (rc) return rc;
+  return dispatch<false>("mdb_gemm_f16", g, kp, geglu, st);
+}
 
-  int splits = g->splits > 1 ? g->splits : 1;
-  if (g->ln_u != nullptr) splits = 1;  // the correction is applied by the CTA that holds the whole K range
-  if (g->splits == 0 && !geglu && !pair && g->ln_u == nullptr) {
-    // automatic split-K: a power of two up to 8 (reduced inside a thread-block cluster through DSMEM) that brings
-    // the grid to about one CTA per SM while every split keeps at least 16 K chunks (below that the cluster
-    // reduction costs more than the extra CTAs gain)
-    const long long tiles = (long long)m_tiles * ((g->n + bn - 1) / bn);
-    if (tiles < 100)
-      for (int c = 8; c >= 2; c >>= 1)
-        if (tiles * c <= kNumSms && kp.k_chunks / c >= 16) {
-          splits = c;
-          break;
-        }
+extern "C" int mdb_conv3x3_igemm_f16(const mdb_gemm_desc* g, mdb_stream_t stream) {
+  const char* fn = "mdb_conv3x3_igemm_f16";
+  MDB_REQUIRE(g != nullptr, "%s: null descriptor", fn);
+  MDB_REQUIRE(g->conv == 1 || g->conv == 2, "%s: conv must be the stride, 1 or 2 (got %d)", fn, g->conv);
+  MDB_REQUIRE(g->a && g->b && g->d, "%s: null operand", fn);
+  MDB_REQUIRE(g->nb > 0 && g->h > 0 && g->w > 0 && g->c > 0 && g->c % kBK == 0 && g->k == 9 * g->c,
+              "%s: needs nb, h, w > 0, c %% 64 == 0 and k == 9c (nb=%d h=%d w=%d c=%d k=%d)", fn, g->nb, g->h, g->w, g->c,
+              g->k);
+  const int cs = g->conv;
+  const int ho = (g->h - 1) / cs + 1, wo = (g->w - 1) / cs + 1;
+  MDB_REQUIRE(g->m == g->nb * ho * wo && g->n > 0, "%s: m=%d must be nb*ho*wo=%d and n=%d > 0", fn, g->m,
+              g->nb * ho * wo, g->n);
+  MDB_REQUIRE(g->epilogue == MDB_EPI_NONE && g->ln_u == nullptr, "%s: no GEGLU epilogue or folded LayerNorm", fn);
+  // two sources: channels [0, k1) of every pixel from a, [k1, c) from a2 (a fused torch.cat along channels)
+  const int c1 = g->a2 ? g->k1 : g->c;
+  MDB_REQUIRE(c1 > 0 && c1 % kBK == 0 && (g->a2 ? c1 < g->c : c1 == g->c),
+              "%s: with a2, k1 (the channels taken from a) must be a multiple of 64 below c (k1=%d c=%d)", fn, c1, g->c);
+  const long long lda = g->lda > 0 ? g->lda : c1, lda2 = g->lda2 > 0 ? g->lda2 : g->c - c1;
+  MDB_REQUIRE(lda >= c1 && lda % 8 == 0 && (!g->a2 || (lda2 >= g->c - c1 && lda2 % 8 == 0)),
+              "%s: the pixel strides lda / lda2 must cover their channels and be multiples of 8 (lda=%lld lda2=%lld)", fn,
+              lda, lda2);
+  MDB_REQUIRE(g->ldd >= g->n && g->ldd % 8 == 0 && (reinterpret_cast<uintptr_t>(g->d) & 15) == 0,
+              "%s: D must be 16B aligned with ldd %% 8 == 0 and ldd >= n (ldd=%lld)", fn, (long long)g->ldd);
+  if (g->bias) {
+    MDB_REQUIRE((reinterpret_cast<uintptr_t>(g->bias) & 15) == 0 && g->bias_batch_stride % 4 == 0,
+                "%s: bias must be 16B aligned with bias_batch_stride %% 4 == 0", fn);
   }
-  if (splits > kp.k_chunks) splits = kp.k_chunks;
-  if (geglu || pair) splits = 1;
-  kp.chunks_per_split = (kp.k_chunks + splits - 1) / splits;
-  splits = (kp.k_chunks + kp.chunks_per_split - 1) / kp.chunks_per_split;  // no empty splits
-  kp.splits = splits;
-  kp.ws = g->splitk_ws;
-  // 2, 4 or 8 splits: the partners form a thread-block cluster and reduce through DSMEM (one kernel);
-  // other counts go through the global fp32 workspace + finalize kernel.
-  kp.cluster_reduce = (!geglu && (splits == 2 || splits == 4 || splits == 8)) ? 1 : 0;
-  if (splits > 1 && !kp.cluster_reduce) {
-    MDB_REQUIRE(g->splitk_ws != nullptr, "mdb_gemm_f16: splits > 1 needs splitk_ws");
+  if (g->residual) {
+    MDB_REQUIRE(g->ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(g->residual) & 15) == 0,
+                "%s: residual must be 16B aligned with ldr %% 8 == 0", fn);
   }
-
-  dim3 grid(m_tiles, (g->n + bn - 1) / bn, splits);
-  const bool deep = (long long)grid.x * grid.y * grid.z <= kNumSms && kp.chunks_per_split >= 12;
-  if (pair) {
-    if (bn == 256) rc = geglu ? launch_gemm<256, true, 4>(kp, grid, st) : launch_gemm<256, false, 4>(kp, grid, st);
-    else if (bn == 160) rc = launch_gemm<160, false, 6>(kp, grid, st);
-    else rc = launch_gemm<128, false, 6>(kp, grid, st);
-    return rc;
-  }
-  if (geglu) rc = launch_gemm<128, true, 3>(kp, grid, st);
-  else if (bn == 160) rc = deep ? launch_gemm<160, false, 6>(kp, grid, st) : launch_gemm<160, false, 3>(kp, grid, st);
-  else if (bn == 80) rc = deep ? launch_gemm<80, false, 8>(kp, grid, st) : launch_gemm<80, false, 3>(kp, grid, st);
-  else rc = deep ? launch_gemm<128, false, 6>(kp, grid, st) : launch_gemm<128, false, 3>(kp, grid, st);
+  GemmKParams kp;
+  memset(&kp, 0, sizeof(kp));
+  kp.d = static_cast<__half*>(g->d);
+  kp.ldd = g->ldd;
+  kp.bias = g->bias;
+  kp.bias_batch_stride = g->bias_batch_stride;
+  kp.rows_per_batch = g->rows_per_batch > 0 ? g->rows_per_batch : 1;
+  kp.residual = static_cast<const __half*>(g->residual);
+  kp.ldr = g->ldr;
+  kp.m = g->m;
+  kp.n = g->n;
+  kp.k_chunks = g->k / kBK;
+  kp.conv = 1;
+  kp.chunks_per_tap = g->c / kBK;
+  kp.k1_chunks = c1 / kBK;
+  kp.w = wo;
+  kp.hw = ho * wo;
+  kp.cs = cs;
+  int rc = tmap_nhwc_im2col(&kp.tmA, g->a, c1, g->w, g->h, g->nb, lda, kBM, cs);
   if (rc) return rc;
-  if (splits > 1 && !kp.cluster_reduce) {
-    const long long total = ((long long)g->m * g->n + 3) / 4;
-    int blocks = (int)((total + 255) / 256);
-    if (blocks > kNumSms * 8) blocks = kNumSms * 8;
-    MDB_CHECK_CUDA(launch_pdl(splitk_finalize_kernel, dim3(blocks), dim3(256), 0, st, kp));
-    count_launch();
-  }
-  return MDB_OK;
+  if (g->a2 && (rc = tmap_nhwc_im2col(&kp.tmA2, g->a2, g->c - c1, g->w, g->h, g->nb, lda2, kBM, cs))) return rc;
+  return dispatch<true>(fn, g, kp, false, static_cast<cudaStream_t>(stream));
 }

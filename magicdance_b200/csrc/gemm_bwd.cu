@@ -53,8 +53,12 @@ __device__ __forceinline__ void gb_put(const GemmBwdKParams& p, long long row, i
   else gb_store2(p.out[1], row, col - p.split_col, v0, v1);
 }
 
-template <int TA>
-__global__ void __launch_bounds__(kWsThreads, 2) gemm_bwd_kernel(const __grid_constant__ GemmBwdKParams p) {
+// IM2COL (conv only, any latent size): the pixel operands come from TMA im2col loads (tmap_nhwc_im2col) that walk the
+// tile's pixels across row and image boundaries.  TA = 0: 128 input pixels of dD per load (stride 1), the window corner
+// (x - 1, y - 1) with offsets (2 - kw, 2 - kh), i.e. output pixel (y + 1 - kh, x + 1 - kw).  TA = 1: 64 output pixels
+// of the forward's A per load, offsets (kw, kh) as in the forward, channels [0, k1) from tmB and the rest from tmB2.
+template <int TA, bool IM2COL>
+__device__ __forceinline__ void gemm_bwd_body(const GemmBwdKParams& p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kGbStages];
   __shared__ __align__(8) uint64_t empty_bar[kGbStages];
@@ -99,7 +103,8 @@ __global__ void __launch_bounds__(kWsThreads, 2) gemm_bwd_kernel(const __grid_co
             tap = kc / p.chunks_per_tap;
             nc = kc - tap * p.chunks_per_tap;
             const int kh = tap / 3, kw = tap - kh * 3;
-            tma_load_4d(sa, &p.tmD, &full_bar[s], nc * 64, x0 + 1 - kw, y0 + 1 - kh, b0);
+            if constexpr (IM2COL) tma_load_im2col_4d(sa, &p.tmD, &full_bar[s], nc * 64, x0 - 1, y0 - 1, b0, 2 - kw, 2 - kh);
+            else tma_load_4d(sa, &p.tmD, &full_bar[s], nc * 64, x0 + 1 - kw, y0 + 1 - kh, b0);
           } else {
             tma_load_2d(sa, &p.tmD, &full_bar[s], kc * 64, r0);
           }
@@ -116,7 +121,15 @@ __global__ void __launch_bounds__(kWsThreads, 2) gemm_bwd_kernel(const __grid_co
               const int kh = tap / 3, kw = tap - kh * 3;
               const int bb = m / p.hw, rem = m - bb * p.hw;
               const int yy = rem / p.w, xx = rem - yy * p.w;
-              tma_load_4d(sb + j * kGbChunk, &p.tmB, &full_bar[s], cc, p.cs * xx + kw - 1, p.cs * yy + kh - 1, bb);
+              if constexpr (IM2COL) {
+                if (cc < p.k1)
+                  tma_load_im2col_4d(sb + j * kGbChunk, &p.tmB, &full_bar[s], cc, p.cs * xx - 1, p.cs * yy - 1, bb, kw, kh);
+                else
+                  tma_load_im2col_4d(sb + j * kGbChunk, &p.tmB2, &full_bar[s], cc - p.k1, p.cs * xx - 1, p.cs * yy - 1, bb,
+                                     kw, kh);
+              } else {
+                tma_load_4d(sb + j * kGbChunk, &p.tmB, &full_bar[s], cc, p.cs * xx + kw - 1, p.cs * yy + kh - 1, bb);
+              }
             } else if (col < p.k1) {
               tma_load_2d(sb + j * kGbChunk, &p.tmB, &full_bar[s], col, m);
             } else {
@@ -169,6 +182,16 @@ __global__ void __launch_bounds__(kWsThreads, 2) gemm_bwd_kernel(const __grid_co
         gb_put(p, row, col, acc[j], acc[j + 1]);
     }
   }
+}
+
+template <int TA>
+__global__ void __launch_bounds__(kWsThreads, 2) gemm_bwd_kernel(const __grid_constant__ GemmBwdKParams p) {
+  gemm_bwd_body<TA, false>(p);
+}
+
+template <int TA>
+__global__ void __launch_bounds__(kWsThreads, 2) gemm_bwd_igemm_kernel(const __grid_constant__ GemmBwdKParams p) {
+  gemm_bwd_body<TA, true>(p);
 }
 
 // the split reduction's second pass: slabs summed in split order, then the destination's dtype / accumulate
@@ -289,51 +312,68 @@ static bool out_ok(const void* p, long long ld, int dtype) {
   return (reinterpret_cast<uintptr_t>(p) & 15) == 0 && ld % 8 == 0 && (dtype == MDB_DTYPE_F16 || dtype == MDB_DTYPE_F32);
 }
 
-static int plan_bwd(const mdb_gemm_bwd_desc* g, GbPlan* pl) {
-  MDB_REQUIRE(g != nullptr, "mdb_gemm_bwd_f16: null descriptor");
+// igemm: the conv at any latent size (mdb_conv3x3_igemm_bwd_f16): dB and stride-1 dA through im2col loads, one or
+// two sources; fn names the entry point in messages
+static int plan_bwd(const mdb_gemm_bwd_desc* g, GbPlan* pl, bool igemm, const char* fn) {
+  MDB_REQUIRE(g != nullptr, "%s: null descriptor", fn);
   const mdb_gemm_desc* f = &g->fwd;
   memset(pl, 0, sizeof(*pl));
   MDB_REQUIRE(f->epilogue == MDB_EPI_NONE,
-              "mdb_gemm_bwd_f16: the GEGLU epilogue has no backward here (differentiate the plain GEMM and the "
-              "activation separately)");
-  MDB_REQUIRE(f->ln_u == nullptr, "mdb_gemm_bwd_f16: the folded LayerNorm (ln_u) has no backward here");
-  MDB_REQUIRE(f->m > 0 && f->n > 0 && f->k > 0 && f->k % 64 == 0, "mdb_gemm_bwd_f16: bad shape m=%d n=%d k=%d",
+              "%s: the GEGLU epilogue has no backward here (differentiate the plain GEMM and the "
+              "activation separately)", fn);
+  MDB_REQUIRE(f->ln_u == nullptr, "%s: the folded LayerNorm (ln_u) has no backward here", fn);
+  MDB_REQUIRE(f->m > 0 && f->n > 0 && f->k > 0 && f->k % 64 == 0, "%s: bad shape m=%d n=%d k=%d", fn,
               f->m, f->n, f->k);
   MDB_REQUIRE(g->dd != nullptr && g->lddd % 8 == 0 && g->lddd >= f->n && (reinterpret_cast<uintptr_t>(g->dd) & 15) == 0,
-              "mdb_gemm_bwd_f16: dd must be 16B aligned with lddd %% 8 == 0 and lddd >= n (lddd=%lld)",
+              "%s: dd must be 16B aligned with lddd %% 8 == 0 and lddd >= n (lddd=%lld)", fn,
               (long long)g->lddd);
-  MDB_REQUIRE(g->splits >= 0 && f->splits >= 0, "mdb_gemm_bwd_f16: negative split count");
+  MDB_REQUIRE(g->splits >= 0 && f->splits >= 0, "%s: negative split count", fn);
   pl->da = g->da != nullptr || g->da2 != nullptr;
   pl->db = g->db != nullptr;
   pl->dbias = g->dbias != nullptr;
-  if (g->da) MDB_REQUIRE(out_ok(g->da, g->ldda, g->da_dtype), "mdb_gemm_bwd_f16: da must be 16B aligned, ldda %% 8 == 0, dtype 0|1");
-  if (g->da2) MDB_REQUIRE(out_ok(g->da2, g->ldda2, g->da2_dtype), "mdb_gemm_bwd_f16: da2 must be 16B aligned, ldda2 %% 8 == 0, dtype 0|1");
-  if (g->db) MDB_REQUIRE(out_ok(g->db, g->lddb, g->db_dtype), "mdb_gemm_bwd_f16: db must be 16B aligned, lddb %% 8 == 0, dtype 0|1");
-  if (pl->da) MDB_REQUIRE(f->b != nullptr && f->ldb % 8 == 0, "mdb_gemm_bwd_f16: dA needs the forward's b (ldb %% 8 == 0)");
-  if (pl->db) MDB_REQUIRE(f->a != nullptr, "mdb_gemm_bwd_f16: dB needs the forward's a");
+  if (g->da) MDB_REQUIRE(out_ok(g->da, g->ldda, g->da_dtype), "%s: da must be 16B aligned, ldda %% 8 == 0, dtype 0|1", fn);
+  if (g->da2) MDB_REQUIRE(out_ok(g->da2, g->ldda2, g->da2_dtype), "%s: da2 must be 16B aligned, ldda2 %% 8 == 0, dtype 0|1", fn);
+  if (g->db) MDB_REQUIRE(out_ok(g->db, g->lddb, g->db_dtype), "%s: db must be 16B aligned, lddb %% 8 == 0, dtype 0|1", fn);
+  if (pl->da) MDB_REQUIRE(f->b != nullptr && f->ldb % 8 == 0, "%s: dA needs the forward's b (ldb %% 8 == 0)", fn);
+  if (pl->db) MDB_REQUIRE(f->a != nullptr, "%s: dB needs the forward's a", fn);
   if (f->bias_batch_stride != 0)
     MDB_REQUIRE(f->rows_per_batch > 0 && f->bias_batch_stride >= f->n,
-                "mdb_gemm_bwd_f16: a per-batch bias needs rows_per_batch > 0 and bias_batch_stride >= n");
+                "%s: a per-batch bias needs rows_per_batch > 0 and bias_batch_stride >= n", fn);
   pl->m = f->m;
+  if (igemm) MDB_REQUIRE(f->conv != 0, "%s: conv must be the stride, 1 or 2 (got 0)", fn);
   if (f->conv) {
-    MDB_REQUIRE(f->conv == 1 || f->conv == 2, "mdb_gemm_bwd_f16: conv must be 1 or 2 (stride), got %d", f->conv);
-    MDB_REQUIRE(f->a2 == nullptr, "mdb_gemm_bwd_f16: conv mode takes a single source");
+    MDB_REQUIRE(f->conv == 1 || f->conv == 2, "%s: conv must be 1 or 2 (stride), got %d", fn, f->conv);
+    MDB_REQUIRE(igemm || f->a2 == nullptr, "%s: conv mode takes a single source", fn);
     MDB_REQUIRE(f->c % 64 == 0 && f->k == 9 * f->c && f->nb > 0 && f->h > 0 && f->w > 0,
-                "mdb_gemm_bwd_f16: conv needs c %% 64 == 0 and k == 9c (c=%d k=%d)", f->c, f->k);
+                "%s: conv needs c %% 64 == 0 and k == 9c (c=%d k=%d)", fn, f->c, f->k);
     pl->cs = f->conv;
     pl->ho = (f->h - 1) / pl->cs + 1;
     pl->wo = (f->w - 1) / pl->cs + 1;
-    MDB_REQUIRE(f->m == f->nb * pl->ho * pl->wo, "mdb_gemm_bwd_f16: conv m != nb*ho*wo");
-    if (pl->da) MDB_REQUIRE(g->da != nullptr && g->da2 == nullptr, "mdb_gemm_bwd_f16: conv dA goes to da only");
-    // pixels that do not form TMA boxes take the column path
+    MDB_REQUIRE(f->m == f->nb * pl->ho * pl->wo, "%s: conv m != nb*ho*wo", fn);
+    if (igemm) {
+      // two sources: channels [0, k1) of every pixel from a (and dA to da), [k1, c) from a2 (dA to da2)
+      const int c1 = f->a2 ? f->k1 : f->c;
+      MDB_REQUIRE(c1 > 0 && c1 % 64 == 0 && (f->a2 ? c1 < f->c : c1 == f->c),
+                  "%s: with a2, k1 (the channels taken from a) must be a multiple of 64 below c (k1=%d c=%d)", fn, c1,
+                  f->c);
+      const long long lda = f->lda > 0 ? f->lda : c1, lda2 = f->lda2 > 0 ? f->lda2 : f->c - c1;
+      if (pl->db)
+        MDB_REQUIRE(lda >= c1 && lda % 8 == 0 && (!f->a2 || (lda2 >= f->c - c1 && lda2 % 8 == 0)),
+                    "%s: the pixel strides lda / lda2 must cover their channels and be multiples of 8", fn);
+      MDB_REQUIRE(g->da2 == nullptr || f->a2 != nullptr, "%s: da2 without a second source", fn);
+      MDB_REQUIRE(!(pl->da && f->a2 && pl->cs == 2), "%s: stride-2 dA of a two-source conv is not supported", fn);
+    } else if (pl->da) {
+      MDB_REQUIRE(g->da != nullptr && g->da2 == nullptr, "%s: conv dA goes to da only", fn);
+    }
+    // pixels that do not form TMA boxes take the column path (igemm: only stride-2 dA, im2col loads otherwise)
     uint32_t box[4];
-    pl->da_col = pl->cs == 2 || pixel_box(f->h, f->w, 1, kGbM, false, box) != kBoxOk;
-    pl->db_col = pixel_box(pl->ho, pl->wo, pl->cs, 64, false, box) != kBoxOk;
+    pl->da_col = pl->cs == 2 || (!igemm && pixel_box(f->h, f->w, 1, kGbM, false, box) != kBoxOk);
+    pl->db_col = !igemm && pixel_box(pl->ho, pl->wo, pl->cs, 64, false, box) != kBoxOk;
   } else {
     const int k1 = f->a2 ? f->k1 : f->k;
-    MDB_REQUIRE(k1 % 64 == 0 && k1 > 0 && k1 <= f->k, "mdb_gemm_bwd_f16: k1=%d must be a multiple of 64 within K", k1);
-    if (pl->db) MDB_REQUIRE(f->lda % 8 == 0 && (!f->a2 || f->lda2 % 8 == 0), "mdb_gemm_bwd_f16: lda %% 8 == 0");
-    MDB_REQUIRE(g->da2 == nullptr || f->a2 != nullptr, "mdb_gemm_bwd_f16: da2 without a second source");
+    MDB_REQUIRE(k1 % 64 == 0 && k1 > 0 && k1 <= f->k, "%s: k1=%d must be a multiple of 64 within K", fn, k1);
+    if (pl->db) MDB_REQUIRE(f->lda % 8 == 0 && (!f->a2 || f->lda2 % 8 == 0), "%s: lda %% 8 == 0", fn);
+    MDB_REQUIRE(g->da2 == nullptr || f->a2 != nullptr, "%s: da2 without a second source", fn);
   }
   long long ws = 0;
   const long long k_tiles = (f->k + kGbN - 1) / kGbN;
@@ -366,18 +406,23 @@ static int plan_bwd(const mdb_gemm_bwd_desc* g, GbPlan* pl) {
   return MDB_OK;
 }
 
-static int launch_bwd_gemm(int ta, GemmBwdKParams& kp, int tiles_x, int splits, int cps, cudaStream_t st) {
+template <auto kern>
+static int launch_bwd_kernel(const GemmBwdKParams& kp, dim3 grid, cudaStream_t st) {
+  if (int rc = set_max_dyn_smem<kern>(kGbSmem)) return rc;
+  MDB_CHECK_CUDA(launch_pdl(kern, grid, dim3(kWsThreads), kGbSmem, st, kp));
+  return MDB_OK;
+}
+
+static int launch_bwd_gemm(int ta, GemmBwdKParams& kp, int tiles_x, int splits, int cps, cudaStream_t st,
+                           bool igemm = false) {
   kp.splits = splits;
   kp.chunks_per_split = cps;
   const dim3 grid(tiles_x, (kp.cols + kGbN - 1) / kGbN, splits);
-  int rc;
-  if (ta == 0) {
-    if ((rc = set_max_dyn_smem<gemm_bwd_kernel<0>>(kGbSmem))) return rc;
-    MDB_CHECK_CUDA(launch_pdl(gemm_bwd_kernel<0>, grid, dim3(kWsThreads), kGbSmem, st, kp));
-  } else {
-    if ((rc = set_max_dyn_smem<gemm_bwd_kernel<1>>(kGbSmem))) return rc;
-    MDB_CHECK_CUDA(launch_pdl(gemm_bwd_kernel<1>, grid, dim3(kWsThreads), kGbSmem, st, kp));
-  }
+  const int rc = igemm ? (ta == 0 ? launch_bwd_kernel<gemm_bwd_igemm_kernel<0>>(kp, grid, st)
+                                  : launch_bwd_kernel<gemm_bwd_igemm_kernel<1>>(kp, grid, st))
+                       : (ta == 0 ? launch_bwd_kernel<gemm_bwd_kernel<0>>(kp, grid, st)
+                                  : launch_bwd_kernel<gemm_bwd_kernel<1>>(kp, grid, st));
+  if (rc) return rc;
   count_launch();
   if (splits > 1) {
     const long long pairs = static_cast<long long>(kp.rows) * kp.cols / 2;
@@ -388,7 +433,7 @@ static int launch_bwd_gemm(int ta, GemmBwdKParams& kp, int tiles_x, int splits, 
   return MDB_OK;
 }
 
-static int run_da(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st) {
+static int run_da(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st, bool igemm = false) {
   const mdb_gemm_desc* f = &g->fwd;
   GemmBwdKParams kp;
   memset(&kp, 0, sizeof(kp));
@@ -398,9 +443,13 @@ static int run_da(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st)
   kp.cols = f->k;
   int tiles_x;
   if (f->conv && !pl.da_col) {  // stride 1, implicit: the row tiles are input pixels
-    uint32_t box[4];
-    pixel_box(f->h, f->w, 1, kGbM, false, box);
-    if ((rc = tmap_nhwc(&kp.tmD, g->dd, f->n, f->w, f->h, f->nb, g->lddd, box, 1))) return rc;
+    if (igemm) {
+      if ((rc = tmap_nhwc_im2col(&kp.tmD, g->dd, f->n, f->w, f->h, f->nb, g->lddd, kGbM, 1))) return rc;
+    } else {
+      uint32_t box[4];
+      pixel_box(f->h, f->w, 1, kGbM, false, box);
+      if ((rc = tmap_nhwc(&kp.tmD, g->dd, f->n, f->w, f->h, f->nb, g->lddd, box, 1))) return rc;
+    }
     kp.conv = 1;
     kp.chunks_per_tap = (f->n + 63) / 64;
     kp.chunks = 9 * kp.chunks_per_tap;
@@ -412,6 +461,10 @@ static int run_da(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st)
     kp.cols = f->c;
     kp.out[0] = gb_out(g->da, g->ldda, g->da_dtype, g->da_accumulate);
     kp.split_col = f->c;
+    if (igemm && f->a2) {  // channels [k1, c) of every input pixel are the second source's
+      kp.out[1] = gb_out(g->da2, g->ldda2, g->da2_dtype, g->da2_accumulate);
+      kp.split_col = f->k1;
+    }
   } else {
     if ((rc = tmap_rows(&kp.tmD, g->dd, f->n, f->m, g->lddd, 64, kGbM))) return rc;
     kp.chunks = (f->n + 63) / 64;
@@ -427,7 +480,7 @@ static int run_da(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st)
   }
   tiles_x = (kp.rows + kGbM - 1) / kGbM;
   kp.ws = g->ws + pl.da_col_floats;
-  if ((rc = launch_bwd_gemm(0, kp, tiles_x, pl.da_splits, pl.da_cps, st))) return rc;
+  if ((rc = launch_bwd_gemm(0, kp, tiles_x, pl.da_splits, pl.da_cps, st, igemm && kp.conv))) return rc;
   if (pl.da_col) {
     const long long total = static_cast<long long>(f->nb) * f->h * f->w * (f->c / 2);
     const int blocks = static_cast<int>(min((total + 255) / 256, static_cast<long long>(kNumSms) * 16));
@@ -439,14 +492,26 @@ static int run_da(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st)
   return MDB_OK;
 }
 
-static int run_db(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st) {
+static int run_db(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st, bool igemm = false) {
   const mdb_gemm_desc* f = &g->fwd;
   GemmBwdKParams kp;
   memset(&kp, 0, sizeof(kp));
   int rc;
   // dD^T: 64 of N x 64 of M per box, read MN-major
   if ((rc = tmap_rows(&kp.tmD, g->dd, f->n, f->m, g->lddd, 64, 64))) return rc;
-  if (f->conv && !pl.db_col) {  // the forward's shifted pixel boxes, 64 output pixels x 64 channels of one tap
+  if (igemm) {  // 64 output pixels x 64 channels of one tap per im2col load, from a or a2
+    const int c1 = f->a2 ? f->k1 : f->c;
+    if ((rc = tmap_nhwc_im2col(&kp.tmB, f->a, c1, f->w, f->h, f->nb, f->lda > 0 ? f->lda : c1, 64, pl.cs))) return rc;
+    if (f->a2 && (rc = tmap_nhwc_im2col(&kp.tmB2, f->a2, f->c - c1, f->w, f->h, f->nb,
+                                        f->lda2 > 0 ? f->lda2 : f->c - c1, 64, pl.cs)))
+      return rc;
+    kp.conv = 1;
+    kp.c = f->c;
+    kp.k1 = c1;
+    kp.w = pl.wo;
+    kp.hw = pl.ho * pl.wo;
+    kp.cs = pl.cs;
+  } else if (f->conv && !pl.db_col) {  // the forward's shifted pixel boxes, 64 output pixels x 64 channels of one tap
     uint32_t box[4];
     pixel_box(pl.ho, pl.wo, pl.cs, 64, false, box);
     if ((rc = tmap_nhwc(&kp.tmB, f->a, f->c, f->w, f->h, f->nb, f->c, box, pl.cs))) return rc;
@@ -471,7 +536,7 @@ static int run_db(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st)
   kp.out[0] = gb_out(g->db, g->lddb, g->db_dtype, g->db_accumulate);
   kp.split_col = f->k;
   kp.ws = g->ws + pl.db_col_floats;
-  return launch_bwd_gemm(1, kp, (f->n + kGbM - 1) / kGbM, pl.db_splits, pl.db_cps, st);
+  return launch_bwd_gemm(1, kp, (f->n + kGbM - 1) / kGbM, pl.db_splits, pl.db_cps, st, igemm);
 }
 
 static int run_dbias(const mdb_gemm_bwd_desc* g, const GbPlan& pl, cudaStream_t st) {
@@ -497,23 +562,36 @@ int launch_colsum_finalize(const float* ws, int n, int segs, int parts, float* o
 
 using namespace mdb;
 
+static int run_bwd(const mdb_gemm_bwd_desc* g, mdb_stream_t stream, bool igemm, const char* fn, const char* ws_fn) {
+  GbPlan pl;
+  int rc = plan_bwd(g, &pl, igemm, fn);
+  if (rc) return rc;
+  MDB_REQUIRE(pl.ws_floats == 0 || (g->ws != nullptr && (reinterpret_cast<uintptr_t>(g->ws) & 15) == 0),
+              "%s: needs a 16B-aligned workspace of %s() = %lld floats", fn, ws_fn, (long long)pl.ws_floats);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // the phases run one after the other on the stream and share the workspace
+  if (pl.da && (rc = run_da(g, pl, st, igemm))) return rc;
+  if (pl.db && (rc = run_db(g, pl, st, igemm))) return rc;
+  if (pl.dbias && (rc = run_dbias(g, pl, st))) return rc;
+  return MDB_OK;
+}
+
 extern "C" int64_t mdb_gemm_bwd_ws_floats(const mdb_gemm_bwd_desc* g) {
   GbPlan pl;
-  const int rc = plan_bwd(g, &pl);
+  const int rc = plan_bwd(g, &pl, false, "mdb_gemm_bwd_f16");
   return rc ? rc : pl.ws_floats;
 }
 
 extern "C" int mdb_gemm_bwd_f16(const mdb_gemm_bwd_desc* g, mdb_stream_t stream) {
+  return run_bwd(g, stream, false, "mdb_gemm_bwd_f16", "mdb_gemm_bwd_ws_floats");
+}
+
+extern "C" int64_t mdb_conv3x3_igemm_bwd_ws_floats(const mdb_gemm_bwd_desc* g) {
   GbPlan pl;
-  int rc = plan_bwd(g, &pl);
-  if (rc) return rc;
-  MDB_REQUIRE(pl.ws_floats == 0 || (g->ws != nullptr && (reinterpret_cast<uintptr_t>(g->ws) & 15) == 0),
-              "mdb_gemm_bwd_f16: needs a 16B-aligned workspace of mdb_gemm_bwd_ws_floats() = %lld floats",
-              (long long)pl.ws_floats);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // the phases run one after the other on the stream and share the workspace
-  if (pl.da && (rc = run_da(g, pl, st))) return rc;
-  if (pl.db && (rc = run_db(g, pl, st))) return rc;
-  if (pl.dbias && (rc = run_dbias(g, pl, st))) return rc;
-  return MDB_OK;
+  const int rc = plan_bwd(g, &pl, true, "mdb_conv3x3_igemm_bwd_f16");
+  return rc ? rc : pl.ws_floats;
+}
+
+extern "C" int mdb_conv3x3_igemm_bwd_f16(const mdb_gemm_bwd_desc* g, mdb_stream_t stream) {
+  return run_bwd(g, stream, true, "mdb_conv3x3_igemm_bwd_f16", "mdb_conv3x3_igemm_bwd_ws_floats");
 }

@@ -104,6 +104,43 @@ int tmap_nhwc(CUtensorMap* out, const void* base, int c, int w, int h, int nb, l
   return make_tmap_f16(out, base, 4, dims, str, box, cs == 2 ? estr : nullptr);
 }
 
+static PFN_cuTensorMapEncodeIm2col_v12000 g_encode_im2col = nullptr;
+
+int tmap_nhwc_im2col(CUtensorMap* out, const void* base, int c, int w, int h, int nb, long long ld, int pixels,
+                     int cs) {
+  if (g_encode_im2col == nullptr) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &fn, cudaEnableDefault, &qres);
+    if (e != cudaSuccess || fn == nullptr || qres != cudaDriverEntryPointSuccess) {
+      set_error("cuTensorMapEncodeIm2col not available from the driver (%s)", cudaGetErrorString(e));
+      return MDB_ERR_CUDA;
+    }
+    g_encode_im2col = reinterpret_cast<PFN_cuTensorMapEncodeIm2col_v12000>(fn);
+  }
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || ld % 8 != 0) {
+    set_error("TMA im2col map: base %p must be 16-byte aligned and the pixel stride (%lld) a multiple of 8", base, ld);
+    return MDB_ERR_INVALID;
+  }
+  const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)nb};
+  const cuuint64_t str[3] = {(cuuint64_t)ld * 2, (cuuint64_t)ld * w * 2, (cuuint64_t)ld * h * w * 2};
+  // The bounding box of window corners, per image, runs along w from lower[0] to w - 1 + upper[0] (and likewise along
+  // h) in steps of cs: corners -1 .. w - 2 are the (w - 1) / cs + 1 output columns of a pad-1 3x3 conv, and a
+  // corner plus its tap offset (0..2) is the input pixel read, -1 .. w (the halo, zero-filled)
+  const int lower[2] = {-1, -1};
+  const int upper[2] = {-1, -1};
+  const cuuint32_t estr[4] = {1u, (cuuint32_t)cs, (cuuint32_t)cs, 1u};
+  CUresult r = g_encode_im2col(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, str, lower, upper,
+                               64, (cuuint32_t)pixels, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeIm2col failed with CUresult %d (c %d, w %d, h %d, nb %d, %d pixels, stride %d)", (int)r,
+              c, w, h, nb, pixels, cs);
+    return MDB_ERR_CUDA;
+  }
+  return MDB_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // direct 3x3 conv, pad 1, stride 1|2, NHWC fp16, fp32 accumulate.
 // CTA: 8x8 output pixels x 32 output channels; input patch (with halo) and the weight slab for a

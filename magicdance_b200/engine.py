@@ -265,28 +265,20 @@ def tensor_key(t):
     return (t.untyped_storage().data_ptr(), t.storage_offset(), tuple(t.shape), tuple(t.stride()), t._version)
 
 
-_warned_sizes = set()
-
-
 def _igemm_ok(h, w, c):
     """does an h x w x c conv output tile into the implicit-GEMM conv's 128-pixel TMA boxes?  (512x512 and 256x256
-    images do at every level.)  Other sizes work through im2col + GEMM — 9x the activation traffic — so say so once."""
+    images do at every level.)  Other sizes take the same kernels with TMA im2col loads (ops.conv3x3_igemm)."""
     hw = h * w
     if c % 64:
         return False
     # mirrors pixel_box(..., fwd=true) in csrc/gemm.cu
-    ok = ((128 % w == 0 and hw % 128 == 0) or w % 128 == 0) if hw >= 128 else (128 % hw == 0)
-    if not ok and (h, w) not in _warned_sizes:
-        _warned_sizes.add((h, w))
-        import warnings
-        warnings.warn(f"magicdance_b200: a {h}x{w} feature map does not tile into 128-pixel TMA boxes; its 3x3 convs take "
-                      "the slower im2col + GEMM path (latents whose width divides 128 avoid this)", stacklevel=3)
-    return ok
+    return ((128 % w == 0 and hw % 128 == 0) or w % 128 == 0) if hw >= 128 else (128 % hw == 0)
 
 
 def conv3x3(x: Act, w, bias, *, cout, stride=1, residual=None, bias_batch_stride=0) -> Act:
-    """3x3 pad-1 conv, w packed by pack_conv3x3.  Tensor cores (implicit GEMM, else im2col + GEMM) when cin and cout
-    fit their tiles; the direct conv otherwise (few channels in or out: the UNet's conv_in/out, the VAE's ends)."""
+    """3x3 pad-1 conv, w packed by pack_conv3x3.  Tensor cores (implicit GEMM over TMA boxes where the pixels tile into
+    them, over TMA im2col loads at any other size) when cin and cout fit their tiles; the direct conv otherwise (few
+    channels in or out: the UNet's conv_in/out, the VAE's ends)."""
     cin = x.c
     ho, wo = (x.h - 1) // stride + 1, (x.w - 1) // stride + 1
     tc = cout % 8 == 0 and cout >= 64 and cin % 64 == 0
@@ -295,10 +287,9 @@ def conv3x3(x: Act, w, bias, *, cout, stride=1, residual=None, bias_batch_stride
                      residual=residual, conv=(x.b, x.h, x.w, cin), conv_stride=stride)
     elif tc:
         # latent sizes whose rows do not tile into 128-pixel TMA boxes (e.g. 96x64 -> 12x8 at the deepest
-        # level): explicit im2col + the same tensor-core GEMM
-        col = ops.im2col3x3(x.data, batch=x.b, h=x.h, w=x.w, c=cin, stride=stride)
-        y = ops.gemm(col, w, bias=bias, bias_batch_stride=bias_batch_stride, rows_per_batch=ho * wo,
-                     residual=residual)
+        # level): the same wgmma kernel, its activation tiles loaded in TMA im2col mode
+        y = ops.conv3x3_igemm(x.data, w, conv=(x.b, x.h, x.w, cin), conv_stride=stride, bias=bias,
+                              bias_batch_stride=bias_batch_stride, rows_per_batch=ho * wo, residual=residual)
     else:
         assert bias_batch_stride == 0
         y = ops.conv3x3_direct(x.data, w, bias, batch=x.b, h=x.h, w=x.w, cin=cin, cout=cout, stride=stride,
@@ -550,6 +541,8 @@ class DenoiseEngine:
             last = i == len(strides) - 1
             if last and _igemm_ok(h, w, cin):
                 x = ops.gemm(x, wt, bias=bias, conv=(b, h, w, cin))
+            elif last and cin % 64 == 0:  # pixels that do not tile into TMA boxes: TMA im2col loads
+                x = ops.conv3x3_igemm(x, wt, conv=(b, h, w, cin), bias=bias)
             else:
                 x = ops.conv3x3_direct(x, wt, bias, batch=b, h=h, w=w, cin=cin, cout=cout, stride=s, silu=not last)
             h, w = (h + 2 - 3) // s + 1, (w + 2 - 3) // s + 1

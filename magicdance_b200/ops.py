@@ -277,6 +277,153 @@ def gemm_backward(a, w, dd, *, a2=None, conv=None, conv_stride=1, bias_batch_str
     return da, da2, dw, dbias
 
 
+def _fill_igemm_desc(g, x, w, x2, conv, conv_stride):
+    """the A-side fields and m, n, k of a GemmDesc for mdb_conv3x3_igemm_*: x [nb*h*w, k1] (x2 [nb*h*w, c - k1]) with
+    unit channel stride, any pixel stride; returns m"""
+    nb, h, wd, c = conv
+    n, k = w.shape
+    assert conv_stride in (1, 2) and k == 9 * c, (conv, w.shape)
+    assert x.dim() == 2 and x.stride(1) == 1 and x.shape[0] == nb * h * wd, (x.shape, conv)
+    g.conv, g.nb, g.h, g.w, g.c = conv_stride, nb, h, wd, c
+    g.a, g.lda = x.data_ptr(), x.stride(0)
+    if x2 is not None:
+        _chk(x2, torch.float16, "x2")
+        assert x2.dim() == 2 and x2.stride(1) == 1 and x2.shape[0] == x.shape[0] and x.shape[1] + x2.shape[1] == c
+        g.a2, g.lda2, g.k1 = x2.data_ptr(), x2.stride(0), x.shape[1]
+    else:
+        assert x.shape[1] == c, (x.shape, conv)
+        g.k1 = c
+    m = _gemm_m(x, conv, conv_stride, None)
+    g.m, g.n, g.k = m, n, k
+    return m
+
+
+def conv3x3_igemm(x, w, *, conv, conv_stride=1, x2=None, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0,
+                  residual=None, splits=0):
+    """3x3 pad-1 conv of the NHWC activation x ([nb*h*w, c], conv=(nb, h, w, c)) at any size, as an implicit GEMM whose
+    activation tiles come from TMA im2col loads (mdb_conv3x3_igemm_f16); w: [cout, 9c] packed [O][kh][kw][I].  x2: a
+    second source for channels [x.shape[1], c) (the concat is never materialised).  bias / per-batch bias / residual /
+    splits as gemm(); at the sizes gemm(conv=...) takes, the result is bit-equal to it."""
+    lib = _lib.load()
+    _chk(x, torch.float16, "x")
+    _chk(w, torch.float16, "w")
+    g = _lib.GemmDesc()
+    n = w.shape[0]
+    m = _fill_igemm_desc(g, x, w, x2, conv, conv_stride)
+    if out is None:
+        out = torch.empty((m, n), dtype=torch.float16, device=x.device)
+    _chk(out, torch.float16, "out")
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape[0] >= m and out.shape[1] == n, (out.shape, m, n)
+    assert w.stride(1) == 1
+    g.b, g.ldb = w.data_ptr(), w.stride(0)
+    g.d, g.ldd = out.data_ptr(), out.stride(0)
+    if bias is not None:
+        _chk(bias, torch.float32, "bias")
+        g.bias, g.bias_batch_stride, g.rows_per_batch = bias.data_ptr(), bias_batch_stride, rows_per_batch
+    if residual is not None:
+        _chk(residual, torch.float16, "residual")
+        assert residual.dim() == 2 and residual.stride(1) == 1
+        g.residual, g.ldr = residual.data_ptr(), residual.stride(0)
+    g.splits = splits
+    if splits > 1:
+        g.splitk_ws = _workspace("splitk", splits * m * n, torch.float32, x.device).data_ptr()
+    _lib.check(lib.mdb_conv3x3_igemm_f16(C.byref(g), _stream()), "conv3x3_igemm_f16")
+    return out
+
+
+def conv3x3_igemm_backward(x, w, dd, *, conv, conv_stride=1, x2=None, bias_batch_stride=0, rows_per_batch=0,
+                           splits=0, db_splits=0, grads=("a", "b"), da_dtype=torch.float16, db_dtype=torch.float32,
+                           out_da=None, out_da2=None, out_db=None, out_dbias=None, accumulate=()):
+    """Gradients of conv3x3_igemm (mdb_conv3x3_igemm_bwd_f16), in gemm_backward()'s conventions: returns (dx, dx2, dw,
+    dbias); dx is [nb*h*w, x.shape[1]], dx2 the x2 channels', dw [cout, 9c] ([O][kh][kw][I]).  Deterministic."""
+    lib = _lib.load()
+    _chk(x, torch.float16, "x")
+    _chk(w, torch.float16, "w")
+    _chk(dd, torch.float16, "dd")
+    assert dd.dim() == 2 and dd.stride(1) == 1
+    dev = x.device
+    g = _lib.GemmBwdDesc()
+    f = g.fwd
+    n, k = w.shape
+    m = _fill_igemm_desc(f, x, w, x2, conv, conv_stride)
+    assert w.stride(1) == 1 and dd.shape[0] >= m and dd.shape[1] == n, (dd.shape, m, n)
+    f.b, f.ldb = w.data_ptr(), w.stride(0)
+    f.splits = splits
+    f.bias_batch_stride, f.rows_per_batch = bias_batch_stride, rows_per_batch
+    g.dd, g.lddd, g.splits = dd.data_ptr(), dd.stride(0), db_splits
+    acc = set(accumulate)
+    da = da2 = dw = dbias = None
+    if "a" in grads:
+        da = _grad_out(out_da, tuple(x.shape), da_dtype, dev, "out_da")
+        g.da, g.ldda, g.da_dtype, g.da_accumulate = da.data_ptr(), da.stride(0), _DTYPES[da.dtype], "a" in acc
+        if x2 is not None:
+            da2 = _grad_out(out_da2, tuple(x2.shape), da_dtype, dev, "out_da2")
+            g.da2, g.ldda2, g.da2_dtype = da2.data_ptr(), da2.stride(0), _DTYPES[da2.dtype]
+            g.da2_accumulate = "a2" in acc
+    if "b" in grads:
+        dw = _grad_out(out_db, (n, k), db_dtype, dev, "out_db")
+        g.db, g.lddb, g.db_dtype, g.db_accumulate = dw.data_ptr(), dw.stride(0), _DTYPES[dw.dtype], "b" in acc
+    if "bias" in grads:
+        shape = (n,) if bias_batch_stride == 0 else (-(-m // rows_per_batch), bias_batch_stride)
+        dbias = torch.empty(shape, dtype=torch.float32, device=dev) if out_dbias is None else out_dbias
+        _chk(dbias, torch.float32, "out_dbias")
+        assert dbias.is_contiguous() and tuple(dbias.shape) == shape, (dbias.shape, shape)
+        g.dbias, g.dbias_accumulate = dbias.data_ptr(), "bias" in acc
+    need = int(lib.mdb_conv3x3_igemm_bwd_ws_floats(C.byref(g)))
+    if need < 0:
+        _lib.check(need, "conv3x3_igemm_bwd_f16")
+    g.ws = _workspace("gemm_bwd", need, torch.float32, dev).data_ptr()
+    _lib.check(lib.mdb_conv3x3_igemm_bwd_f16(C.byref(g), _stream()), "conv3x3_igemm_bwd_f16")
+    return da, da2, dw, dbias
+
+
+class Conv3x3Igemm(torch.autograd.Function):
+    """conv3x3_igemm() as an autograd op, in TcGemm's conventions: w is an fp16 activation-like operand or the packed
+    fp16 copy of the fp32 OIHW parameter w_param (which then receives the fp32 gradient); the bias gets its fp32
+    gradient, the residual dD.  Positional arguments in conv3x3_igemm_ad()'s order."""
+
+    @staticmethod
+    def forward(ctx, x, w, w_param, bias, residual, x2, bias_batch_stride, rows_per_batch, conv, conv_stride, splits):
+        n = w.shape[0]
+        m = _gemm_m(x, conv, conv_stride, None)
+        out = torch.empty((m, (n + 7) // 8 * 8), dtype=torch.float16, device=x.device)[:, :n]
+        conv3x3_igemm(x, w, conv=conv, conv_stride=conv_stride, x2=x2, out=out, bias=bias,
+                      bias_batch_stride=bias_batch_stride, rows_per_batch=rows_per_batch, residual=residual,
+                      splits=splits)
+        ctx.save_for_backward(x, w, w_param, x2)
+        ctx.kw = dict(conv=conv, conv_stride=conv_stride, bias_batch_stride=bias_batch_stride,
+                      rows_per_batch=rows_per_batch)
+        ctx.bias_shape = None if bias is None else bias.shape
+        ctx.has_residual = residual is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        x, w, w_param, x2 = ctx.saved_tensors
+        dd = _rows8(dout)
+        need = ctx.needs_input_grad
+        grads = [nm for nm, want in (("a", need[0] or need[5]), ("b", need[1] or need[2]), ("bias", need[3])) if want]
+        dx, dx2, dw, dbias = conv3x3_igemm_backward(
+            x, w, dd, x2=x2, grads=grads, db_dtype=torch.float32 if w_param is not None else torch.float16, **ctx.kw)
+        g_w = g_wp = None
+        if dw is not None:
+            if w_param is not None:  # Conv2d OIHW: the kernel's [O][kh][kw][I] rows, viewed
+                g_wp = dw.view(w_param.shape[0], 3, 3, -1).permute(0, 3, 1, 2)
+            else:
+                g_w = dw
+        g_bias = dbias.view(ctx.bias_shape) if dbias is not None else None
+        g_res = dout if ctx.has_residual else None
+        return dx, g_w, g_wp, g_bias, g_res, dx2, None, None, None, None, None
+
+
+def conv3x3_igemm_ad(x, w, *, w_param=None, bias=None, bias_batch_stride=0, rows_per_batch=0, residual=None, x2=None,
+                     conv, conv_stride=1, splits=0):
+    """Differentiable conv3x3_igemm() (Conv3x3Igemm): the training forward's 3x3 conv at latent sizes whose pixels do
+    not tile into the box path's 128-pixel TMA boxes"""
+    return Conv3x3Igemm.apply(x, w, w_param, bias, residual, x2, bias_batch_stride, rows_per_batch, conv, conv_stride,
+                              splits)
+
+
 def _rows8(t):
     """t as a [rows, cols] fp16 matrix whose row stride is a multiple of 8 (the kernels' alignment), copied if not"""
     if t.stride(1) == 1 and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0:

@@ -227,25 +227,30 @@ class TrainNet:
 # layers and blocks
 # ------------------------------------------------------------------------------------------------
 def check_latent_size(cfg, h, w):
-    """The training path runs every tensor-core 3x3 conv as an implicit GEMM: the latent must tile into its 128-pixel
-    boxes at every level (16x16, 32x32 and 64x64 latents do: 128, 256 and 512 pixel images)."""
+    """The training forward halves the latent at every level but the last and concatenates each output block's input
+    with the skip of the same size, so both sides must be divisible by 2^(levels - 1) (8: 64x64, 112x64, 40x24 ...).
+    Its tensor-core 3x3 convs run as implicit GEMMs over TMA boxes where the pixels tile into them and over TMA im2col
+    loads otherwise, so any such size works."""
     levels = len(cfg.channel_mult)
-    ok = h % (1 << (levels - 1)) == 0 and w % (1 << (levels - 1)) == 0
-    ok = ok and all(_igemm_ok(h >> l, w >> l, 64) for l in range(levels))
-    if not ok:
-        raise ValueError(f"magicdance_b200: the training forward supports latents whose 3x3 convs tile into the implicit "
-                         f"GEMM at every level (16x16, 32x32, 64x64); {h}x{w} does not")
+    if h <= 0 or w <= 0 or h % (1 << (levels - 1)) or w % (1 << (levels - 1)):
+        raise ValueError(f"magicdance_b200: the training forward supports latents whose sides are multiples of "
+                         f"{1 << (levels - 1)} (one halving per level); {h}x{w} is not")
 
 
 def _conv3x3(x: Act, w, cout, *, stride=1, bias=None, residual=None, bias_batch_stride=0) -> Act:
-    """engine.conv3x3 on the autograd ops (implicit GEMM, else the direct conv for few channels in or out)"""
+    """engine.conv3x3 on the autograd ops (implicit GEMM over TMA boxes or TMA im2col loads, else the direct conv for
+    few channels in or out)"""
     w16, wp = w
     cin = x.c
     ho, wo = (x.h - 1) // stride + 1, (x.w - 1) // stride + 1
     if cout % 8 == 0 and cout >= 64 and cin % 64 == 0:
-        assert _igemm_ok(ho, wo, cin), (ho, wo, cin)  # check_latent_size() ran before
-        y = ops.tc_gemm(x.data, w16, w_param=wp, bias=bias, bias_batch_stride=bias_batch_stride,
-                        rows_per_batch=ho * wo, residual=residual, conv=(x.b, x.h, x.w, cin), conv_stride=stride)
+        if _igemm_ok(ho, wo, cin):
+            y = ops.tc_gemm(x.data, w16, w_param=wp, bias=bias, bias_batch_stride=bias_batch_stride,
+                            rows_per_batch=ho * wo, residual=residual, conv=(x.b, x.h, x.w, cin), conv_stride=stride)
+        else:
+            y = ops.conv3x3_igemm_ad(x.data, w16, w_param=wp, bias=bias, bias_batch_stride=bias_batch_stride,
+                                     rows_per_batch=ho * wo, residual=residual, conv=(x.b, x.h, x.w, cin),
+                                     conv_stride=stride)
     else:
         assert bias_batch_stride == 0
         y = ops.direct_conv3x3(x.data, w16, w_param=wp, bias=bias, residual=residual, batch=x.b, h=x.h, w=x.w,
@@ -400,13 +405,16 @@ def appearance_write(net: TrainNet, ref16: Act, t, text):
 
 
 def hint_features(net: TrainNet, pose_map):
-    """ControlNet.input_hint_block (cldm.py:599-615): 7 direct convs + SiLU, the last conv as an implicit GEMM"""
+    """ControlNet.input_hint_block (cldm.py:599-615): 7 direct convs + SiLU, the last conv as an implicit GEMM (over TMA
+    boxes, or TMA im2col loads where the latent's pixels do not tile into them)"""
     b, _, h, w = pose_map.shape
     x = ops.nchw_to_nhwc(pose_map)
     strides = (1, 1, 2, 1, 2, 1, 2, 1)
     for i, (((w16, wp), bias, cin, cout), s) in enumerate(zip(net.hint, strides)):
         if i == len(strides) - 1 and _igemm_ok(h, w, cin):
             x = ops.tc_gemm(x, w16, w_param=wp, bias=bias, conv=(b, h, w, cin))
+        elif i == len(strides) - 1 and cin % 64 == 0:
+            x = ops.conv3x3_igemm_ad(x, w16, w_param=wp, bias=bias, conv=(b, h, w, cin))
         else:
             x = ops.direct_conv3x3(x, w16, w_param=wp, bias=bias, batch=b, h=h, w=w, cin=cin, cout=cout, stride=s,
                                    silu=i != len(strides) - 1)

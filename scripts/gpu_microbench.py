@@ -254,9 +254,43 @@ def direct_bwd_cases():
                      bytes_=10.0 * e)
 
 
+def igemm_case(b, hh, ww, cin, cout, stride=1):
+    """one 3x3 conv (+ bias) four ways: TMA im2col loads, im2col3x3 + GEMM, the TMA-box path where the pixels tile,
+    and cuDNN (fp16 channels-last F.conv2d)"""
+    from magicdance_b200.engine import _igemm_ok
+    x, w, bias = h(b * hh * ww, cin), h(cout, 9 * cin), f(cout)
+    ho, wo = (hh - 1) // stride + 1, (ww - 1) // stride + 1
+    fl = 2.0 * b * ho * wo * cout * 9 * cin
+    conv = (b, hh, ww, cin)
+    tag = f"B={b} {hh}x{ww} {cin}->{cout} s={stride}"
+    timeit(f"im2col-mode TMA  {tag}", lambda: ops.conv3x3_igemm(x, w, conv=conv, conv_stride=stride, bias=bias),
+           flops=fl)
+    timeit(f"im2col3x3+gemm   {tag}", lambda: ops.gemm(ops.im2col3x3(x, batch=b, h=hh, w=ww, c=cin, stride=stride), w,
+                                                        bias=bias), flops=fl)
+    if _igemm_ok(ho, wo, cin):
+        timeit(f"box TMA          {tag}", lambda: ops.gemm(x, w, bias=bias, conv=conv, conv_stride=stride), flops=fl)
+    xc = x.reshape(b, hh, ww, cin).permute(0, 3, 1, 2)
+    wc = w.reshape(cout, 3, 3, cin).permute(0, 3, 1, 2)
+    bh = bias.half()
+    timeit(f"cuDNN            {tag}", lambda: torch.nn.functional.conv2d(xc, wc, bh, padding=1, stride=stride),
+           flops=fl)
+
+
 def main():
     which = sys.argv[1] if len(sys.argv) > 1 else "all"
     ops.ensure_device()
+    if which == "igemm":
+        import subprocess
+        smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True).stdout.strip()
+        print(f"GPU: {torch.cuda.get_device_name()} | nvidia-smi: {smi}", flush=True)
+        # the UNet's 3x3 convs at a 112x64 latent (512x896 portrait), B = 2 (one CFG pair), and a box size for scale
+        for hh, ww, cin, cout in ((112, 64, 320, 320), (28, 16, 640, 640), (14, 8, 1280, 1280), (14, 8, 2560, 1280),
+                                  (56, 32, 960, 320), (64, 64, 320, 320)):
+            igemm_case(2, hh, ww, cin, cout)
+        for hh, ww, c in ((112, 64, 320), (28, 16, 640)):
+            igemm_case(2, hh, ww, c, c, stride=2)
+        return
     if which == "direct_bwd":
         import subprocess
         smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],

@@ -16,7 +16,12 @@ With --stage 1 it measures stage-1 appearance-control pre-training instead (mode
 scripts/appearance_control_pretraining.sh: ControlLDMReferenceOnly, the appearance net trained, the same UNet freeze, its
 time_embed reached by the gradient); no reference FLOP count is taken for it.
 
-    python scripts/train_bench.py [--stage 2] [--batch 4] [--latent 64] [--steps 5] [--warmup 2] [--modes ckpt,plain]
+With --latent-hw HxW (e.g. 112x64: a 512x896 portrait frame) it trains at a latent whose sides need not be equal or
+tile into the implicit-GEMM conv's TMA boxes (those levels' 3x3 convs run on TMA im2col loads); the reference FLOP
+count is for 64x64 and is then not used.
+
+    python scripts/train_bench.py [--stage 2] [--batch 4] [--latent 64 | --latent-hw 112x64] [--steps 5] [--warmup 2]
+                                  [--modes ckpt,plain]
 """
 from __future__ import annotations
 
@@ -68,16 +73,31 @@ def build_model(stage=2):
     return model.to("cuda").train()
 
 
-def run(model, batch, latent, steps, warmup, checkpointing):
+def _inputs_hw(batch, h, w):
+    """synth_inputs' recipe at an h x w latent"""
+    import torch
+    g = torch.Generator().manual_seed(0)
+    u, v = torch.rand(batch, 3, 8 * h, 8 * w, generator=g), torch.rand(batch, 3, 8 * h, 8 * w, generator=g)
+    return {"ref": 0.8 * torch.randn(batch, 4, h, w, generator=g), "pose": torch.where(u > 0.97, v, torch.zeros_like(v)),
+            "context": torch.randn(1, 77, 768, generator=g).expand(batch, -1, -1).contiguous()}
+
+
+def run(model, batch, latent, steps, warmup, checkpointing, latent_hw=None):
     import torch
     from magicdance_b200 import synth
     for net in (n for n in model._nets() if n is not None):
         net.use_checkpoint = checkpointing
     opt = torch.optim.AdamW([p for p in model.parameters() if p.requires_grad], lr=1e-5)
-    inp = {k: v.cuda() for k, v in synth.synth_inputs(batch, latent, seed=0, shared_reference=False).items()}
+    if latent_hw is None:
+        inp = synth.synth_inputs(batch, latent, seed=0, shared_reference=False)
+        h = w = latent
+    else:
+        h, w = latent_hw
+        inp = _inputs_hw(batch, h, w)
+    inp = {k: v.cuda() for k, v in inp.items()}
     g = torch.Generator(device="cuda").manual_seed(0)
     cond = {"c_concat": [inp["pose"]], "c_crossattn": [inp["context"]], "image_control": [inp["ref"]], "wonoise": True}
-    x0 = 0.9 * torch.randn(batch, 4, latent, latent, device="cuda", generator=g)
+    x0 = 0.9 * torch.randn(batch, 4, h, w, device="cuda", generator=g)
 
     def step():
         t = torch.randint(0, 1000, (batch,), device="cuda", generator=g)
@@ -102,7 +122,7 @@ def run(model, batch, latent, steps, warmup, checkpointing):
            "peak_allocated_gib": torch.cuda.max_memory_allocated() / 2 ** 30,
            "algorithmic_tflops_vs_reference_count": REFERENCE_GF_PER_SAMPLE * batch / ms,
            "finite": bool(torch.isfinite(loss))}
-    if model._nets()[2] is None:  # the reference FLOP count is stage 2's
+    if model._nets()[2] is None or latent_hw is not None:  # the reference FLOP count is stage 2's, at 64x64
         del res["algorithmic_tflops_vs_reference_count"]
     del opt
     model.zero_grad(set_to_none=True)
@@ -116,10 +136,12 @@ def main():
                     help="2: appearance-disentangled pose control; 1: appearance-control pre-training")
     ap.add_argument("--batch", type=int, default=4)
     ap.add_argument("--latent", type=int, default=64)
+    ap.add_argument("--latent-hw", default=None, help="HxW: a latent of H rows and W columns instead of --latent")
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--modes", default="ckpt,plain", help="ckpt (activation checkpointing), plain (none)")
     args = ap.parse_args()
+    latent_hw = tuple(int(v) for v in args.latent_hw.lower().split("x")) if args.latent_hw else None
     import torch
     assert torch.cuda.is_available(), "needs an sm_90 GPU"
     name, limit = gpu_info()
@@ -132,9 +154,13 @@ def main():
         out = {"metric": "training samples/s (stage 1 appearance-control pre-training, one GPU)", "device": name,
                "power_limit_w": limit, "batch": args.batch, "latent": args.latent, "steps": args.steps,
                "warmup": args.warmup}
+    if latent_hw is not None:
+        out["latent"] = list(latent_hw)
+        out.pop("reference_gf_per_sample", None)
     for mode in args.modes.split(","):
         try:
-            out[mode] = run(model, args.batch, args.latent, args.steps, args.warmup, checkpointing=mode == "ckpt")
+            out[mode] = run(model, args.batch, args.latent, args.steps, args.warmup, checkpointing=mode == "ckpt",
+                            latent_hw=latent_hw)
         except torch.cuda.OutOfMemoryError:
             model.zero_grad(set_to_none=True)
             torch.cuda.empty_cache()
