@@ -52,6 +52,12 @@ int64_t mdb_abi_struct_bytes(int32_t which);
 #define MDB_TUNE_GEMM_PAIR_MIN_TILES 1 /* grids of >= this many tiles use the one-CTA-per-SM large-grid tiles (128) */
 #define MDB_TUNE_ATTN40_2Q_MIN_CTAS 3  /* d=40 attention grids of >= this many CTAs run two CTAs per SM (512) */
 #define MDB_TUNE_GEMM_BN80_BELOW 4     /* N %% 160 == 0 layers with fewer 160-wide CTAs than this take 80-wide tiles (100) */
+enum {
+  MDB_TUNE_GEMM_SKINNY_CTAS = 5,     /* automatic plan of long-K grids (K >= 4096) of at most half this many tiles:
+                                      * 80-wide tiles, K split up to this many CTAs (96); 0 = the compute-bound plan
+                                      * (powers of two, >= 16 K chunks per split) */
+  MDB_TUNE_GEMM_SPLIT_MIN_CHUNKS = 6 /* ... with at least this many 64-wide K chunks per split (8) */
+};
 int mdb_set_tuning(int32_t key, int32_t value);
 int32_t mdb_get_tuning(int32_t key);
 
@@ -87,8 +93,8 @@ typedef struct mdb_gemm_desc {
   const void* residual;       /* fp16 [M][N] added after bias, may be NULL                        */
   int64_t ldr;
   int32_t m, n, k;
-  int32_t splits;             /* 0: automatic (1, 2, 4 or 8, in-cluster reduction); 1: none; >1: as given */
-  float* splitk_ws;           /* fp32 [splits][M][N] scratch, only for explicit split counts other than 2, 4, 8 */
+  int32_t splits;             /* 0: automatic (1 ... 8, in-cluster reduction); 1: none; >1: as given */
+  float* splitk_ws;           /* fp32 [splits][M][N] scratch, only for explicit split counts above 8 */
   /* LayerNorm over A's rows folded into the GEMM (norm2 -> attn2.to_q of BasicTransformerBlock,
    * attention.py:271,312-314): with B = W diag(gamma) and bias = W beta (+ the layer's own bias) supplied by the
    * caller, ln_u[n] = sum_k B[n][k] makes D = rstd_r (A B^T - mean_r ln_u) + bias equal to LayerNorm(A) W^T + b; K must

@@ -164,6 +164,7 @@ SIGNATURES = {
 _lib = None
 ABI_VERSION = 2
 TUNE_GEMM_PAIR_MIN_TILES, TUNE_ATTN40_2Q_MIN_CTAS, TUNE_GEMM_BN80_BELOW = 1, 3, 4
+TUNE_GEMM_SKINNY_CTAS, TUNE_GEMM_SPLIT_MIN_CHUNKS = 5, 6
 
 
 def library_path() -> str:

@@ -373,13 +373,14 @@ __device__ __forceinline__ void gemm_tc_body(const GemmKParams& p) {
   if constexpr (!GEGLU) {
     if (p.cluster_reduce) {
       // ---- split-K reduction across the cluster through distributed shared memory ----
-      // cluster = the `splits` CTAs of this output tile.  CTA r owns rows [r*R, (r+1)*R) of the tile: it
-      // sums that slice over all partners' parked partials (ld.shared::cluster), applies the epilogue
-      // and stores fp16.  No global workspace, no second kernel.
+      // cluster = the `splits` CTAs of this output tile (2 ... 8).  CTA r owns rows [r*128/S, (r+1)*128/S) of the
+      // tile: it sums that slice over all partners' parked partials in split order (ld.shared::cluster), applies the
+      // epilogue and stores fp16.  No global workspace, no second kernel.
       const int S_ = p.splits;
-      const int R = kBM / S_;
-      const int groups = BN / 8;
       const uint32_t crank = cluster_ctarank();
+      const int r_begin = static_cast<int>(crank) * kBM / S_;
+      const int R = (static_cast<int>(crank) + 1) * kBM / S_ - r_begin;
+      const int groups = BN / 8;
       // this thread's share of the residual is known up front: fetch it before the cluster barrier
       constexpr int kMaxItems = 4;
       uint4 rpre[kMaxItems];
@@ -389,7 +390,7 @@ __device__ __forceinline__ void gemm_tc_body(const GemmKParams& p) {
           const int item = threadIdx.x + q * kWsThreads;
           if (item < R * groups) {
             const int rl = item / groups, cgp = item - rl * groups;
-            const long long row = static_cast<long long>(m0) + static_cast<int>(crank) * R + rl;
+            const long long row = static_cast<long long>(m0) + r_begin + rl;
             const int col0 = n0 + cgp * 8;
             if (row < p.m && col0 + 8 <= p.n) rpre[q] = *reinterpret_cast<const uint4*>(p.residual + row * p.ldr + col0);
           }
@@ -402,7 +403,7 @@ __device__ __forceinline__ void gemm_tc_body(const GemmKParams& p) {
         const int item = threadIdx.x + it_ * kWsThreads;
         if (item >= R * groups) break;
         const int rl = item / groups, cgp = item - rl * groups;
-        const int rt = static_cast<int>(crank) * R + rl;  // row inside the tile
+        const int rt = r_begin + rl;  // row inside the tile
         const long long row = static_cast<long long>(m0) + rt;
         const int col0 = n0 + cgp * 8;
         if (row >= p.m || col0 >= p.n) continue;
@@ -543,6 +544,8 @@ int pixel_box(int ho, int wo, int cs, int rows, bool fwd, uint32_t box[4]) {
 // launch heuristics (mdb_set_tuning)
 static int g_pair_min_tiles = 128;  // smallest grid, in 128-row tile equivalents, that goes to the 256-wide tiles
 static int g_bn80_below = 100;      // N % 160 == 0 layers with fewer 160-wide CTAs than this use 80-wide tiles
+static int g_skinny_ctas = 96;      // long-K grids of at most half this many tiles split K up to this many CTAs (0: off)
+static int g_split_min_chunks = 8;  // ... keeping at least this many K chunks per split
 constexpr int kLongKChunks = 64;    // ... unless K >= 4096 (automatic split-K): then 160-wide tiles and split K
 
 template <auto kern, int BN, int STAGES>
@@ -566,11 +569,16 @@ static int launch_gemm(const GemmKParams& kp, dim3 grid, cudaStream_t st) {
   }
 }
 
-int get_gemm_tuning(int key) { return key == MDB_TUNE_GEMM_PAIR_MIN_TILES ? g_pair_min_tiles : g_bn80_below; }
-void set_gemm_tuning(int key, int value) {
-  if (key == MDB_TUNE_GEMM_PAIR_MIN_TILES) g_pair_min_tiles = value;
-  else g_bn80_below = value;
+static int* gemm_tuning_slot(int key) {
+  switch (key) {
+    case MDB_TUNE_GEMM_PAIR_MIN_TILES: return &g_pair_min_tiles;
+    case MDB_TUNE_GEMM_SKINNY_CTAS: return &g_skinny_ctas;
+    case MDB_TUNE_GEMM_SPLIT_MIN_CHUNKS: return &g_split_min_chunks;
+    default: return &g_bn80_below;
+  }
 }
+int get_gemm_tuning(int key) { return *gemm_tuning_slot(key); }
+void set_gemm_tuning(int key, int value) { *gemm_tuning_slot(key) = value; }
 
 // tile width, split-K and kernel choice for a descriptor validated and A-mapped by the caller: the same rules for the
 // GEMM, the box-path conv and (IM2COL) the conv at any size
@@ -602,9 +610,11 @@ static int dispatch(const char* fn, const mdb_gemm_desc* g, GemmKParams& kp, boo
   } else if (g->n % 160 == 0) {
     // 160-wide tiles unless that leaves most of the SMs idle; then (short K) halve the tile width, or (long K:
     // the weight-streaming 3x3 convs of the 8x8 ... 32x32 levels at one frame) keep the wide tile and split K —
-    // see the automatic split-K below (scripts/gpu_microbench.py times the tile width x split-K choices)
+    // see the automatic split-K below (scripts/gpu_microbench.py times the tile width x split-K choices).  Under the
+    // skinny plan the narrow tile always comes first: it doubles the CTAs that stream distinct weight rows.
     const long long tiles160 = (long long)m_tiles * (g->n / 160) * (g->splits > 1 ? g->splits : 1);
-    const bool wide_split = g->splits == 0 && kp.k_chunks >= kLongKChunks && tiles160 * 2 <= kNumSms;
+    const bool skinny80 = g->splits == 0 && g_skinny_ctas > 0 && kp.k_chunks >= kLongKChunks && tiles160 * 4 <= g_skinny_ctas;
+    const bool wide_split = g->splits == 0 && !skinny80 && kp.k_chunks >= kLongKChunks && tiles160 * 2 <= kNumSms;
     bn = (tiles160 < g_bn80_below && !wide_split) ? 80 : 160;
   } else {
     bn = 128;
@@ -615,16 +625,28 @@ static int dispatch(const char* fn, const mdb_gemm_desc* g, GemmKParams& kp, boo
   int splits = g->splits > 1 ? g->splits : 1;
   if (g->ln_u != nullptr) splits = 1;  // the correction is applied by the CTA that holds the whole K range
   if (g->splits == 0 && !geglu && !pair && g->ln_u == nullptr) {
-    // automatic split-K: a power of two up to 8 (reduced inside a thread-block cluster through DSMEM) that brings
-    // the grid to about one CTA per SM while every split keeps at least 16 K chunks (below that the cluster
-    // reduction costs more than the extra CTAs gain)
     const long long tiles = (long long)m_tiles * ((g->n + bn - 1) / bn);
-    if (tiles < 100)
+    if (g_skinny_ctas > 0 && kp.k_chunks >= kLongKChunks && tiles * 2 <= g_skinny_ctas) {
+      // skinny plan (the 3x3 convs and ff out of the deep levels of a one-frame step, M = 64 ... 512): too few flops
+      // per weight byte to be compute-bound, so what counts is how many SMs stream the weights.  Split K into any
+      // count up to 8 (one cluster, reduced through DSMEM) that keeps the grid within g_skinny_ctas CTAs and every
+      // split at g_split_min_chunks or more.  On H100 (scripts/gpu_microbench.py skinny) 96 CTAs beat 128: clusters
+      // of one-CTA-per-SM tiles do not all fit into the GPCs at once beyond that.  Short K (< 64 chunks) keeps the
+      // plan below: there the fixed cost of a launch dominates and more splits only add reduction work.
+      for (int c = 8; c >= 2; --c)
+        if (tiles * c <= g_skinny_ctas && kp.k_chunks / c >= g_split_min_chunks) {
+          splits = c;
+          break;
+        }
+    } else if (tiles < 100) {
+      // compute-bound plan: a power of two up to 8 that brings the grid to about one CTA per SM while every split
+      // keeps at least 16 K chunks
       for (int c = 8; c >= 2; c >>= 1)
         if (tiles * c <= kNumSms && kp.k_chunks / c >= 16) {
           splits = c;
           break;
         }
+    }
   }
   if (splits > kp.k_chunks) splits = kp.k_chunks;
   if (geglu || pair) splits = 1;
@@ -632,9 +654,9 @@ static int dispatch(const char* fn, const mdb_gemm_desc* g, GemmKParams& kp, boo
   splits = (kp.k_chunks + kp.chunks_per_split - 1) / kp.chunks_per_split;  // no empty splits
   kp.splits = splits;
   kp.ws = g->splitk_ws;
-  // 2, 4 or 8 splits: the partners form a thread-block cluster and reduce through DSMEM (one kernel);
-  // other counts go through the global fp32 workspace + finalize kernel.
-  kp.cluster_reduce = (!geglu && (splits == 2 || splits == 4 || splits == 8)) ? 1 : 0;
+  // 2 ... 8 splits (a portable cluster size): the partners form a thread-block cluster and reduce through DSMEM (one
+  // kernel); more go through the global fp32 workspace + finalize kernel.
+  kp.cluster_reduce = (!geglu && splits >= 2 && splits <= 8) ? 1 : 0;
   if (splits > 1 && !kp.cluster_reduce) {
     MDB_REQUIRE(g->splitk_ws != nullptr, "%s: splits > 1 needs splitk_ws", fn);
   }

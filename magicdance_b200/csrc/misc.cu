@@ -610,6 +610,8 @@ extern "C" int mdb_set_tuning(int32_t key, int32_t value) {
   switch (key) {
     case MDB_TUNE_GEMM_PAIR_MIN_TILES:
     case MDB_TUNE_GEMM_BN80_BELOW:
+    case MDB_TUNE_GEMM_SKINNY_CTAS:
+    case MDB_TUNE_GEMM_SPLIT_MIN_CHUNKS:
       mdb::set_gemm_tuning(key, value);
       return MDB_OK;
     case MDB_TUNE_ATTN40_2Q_MIN_CTAS:

@@ -23,7 +23,8 @@ class tuning:
     mdb_set_tuning) for the duration of the block; tests use it to force a kernel variant onto small problems.
     Launches captured into CUDA graphs keep the variant they were captured with."""
     _KEYS = {"pair_min_tiles": _lib.TUNE_GEMM_PAIR_MIN_TILES,
-             "attn40_2q_min_ctas": _lib.TUNE_ATTN40_2Q_MIN_CTAS, "bn80_below": _lib.TUNE_GEMM_BN80_BELOW}
+             "attn40_2q_min_ctas": _lib.TUNE_ATTN40_2Q_MIN_CTAS, "bn80_below": _lib.TUNE_GEMM_BN80_BELOW,
+             "skinny_ctas": _lib.TUNE_GEMM_SKINNY_CTAS, "split_min_chunks": _lib.TUNE_GEMM_SPLIT_MIN_CHUNKS}
 
     def __init__(self, **kw):
         self.want = {self._KEYS[k]: int(v) for k, v in kw.items() if v is not None}
@@ -155,9 +156,8 @@ def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, re
          a2=None, conv=None, conv_stride=1, splits=0, m=None, ln_u=None, ln_eps=1e-5):
     """D = epilogue(A @ W^T).  a: [M, K1] fp16 (last dim contiguous, row stride arbitrary) or, with
     conv=(nb, h, w, c), an NHWC activation; w: [N, K] fp16; a2: optional second K-range source.
-    splits: 0 = the library picks tile width and split-K (1/2/4/8, reduced inside a thread-block cluster),
-    1 = no split, n = at most n splits (no split is left empty; a count other than 2, 4, 8 goes through an fp32
-    workspace).
+    splits: 0 = the library picks tile width and split-K (1 ... 8, reduced inside a thread-block cluster),
+    1 = no split, n = at most n splits (no split is left empty; a count above 8 goes through an fp32 workspace).
     ln_u: LayerNorm over a's rows folded into the GEMM — w must be W diag(gamma), bias W beta (+ b), ln_u the row sums
     of w (engine.fold_layernorm); D = rstd_r (a w^T - mean_r ln_u) + bias.  Small grids only."""
     lib = _lib.load()
@@ -190,9 +190,9 @@ def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, re
     if TRACE is not None:
         TRACE.append((m, n, k, (tuple(conv) + (conv_stride,)) if conv is not None else None, epilogue, splits,
                       a2.shape[1] if a2 is not None else 0))
-    if splits > 1:
-        # the library rounds the count so that no split is empty (4 splits of 6 K chunks run as 3), and every count
-        # but 2, 4 and 8 reduces through this workspace; with 2, 4 or 8 it reduces in a cluster and ignores it
+    if splits > 8:
+        # the library rounds the count so that no split is empty (12 splits of 20 K chunks run as 10); up to 8 splits
+        # reduce inside a cluster, more through this workspace
         ws = _workspace("splitk", splits * m * n, torch.float32, a.device)
         g.splits, g.splitk_ws = splits, ws.data_ptr()
     else:
@@ -325,7 +325,7 @@ def conv3x3_igemm(x, w, *, conv, conv_stride=1, x2=None, out=None, bias=None, bi
         assert residual.dim() == 2 and residual.stride(1) == 1
         g.residual, g.ldr = residual.data_ptr(), residual.stride(0)
     g.splits = splits
-    if splits > 1:
+    if splits > 8:
         g.splitk_ws = _workspace("splitk", splits * m * n, torch.float32, x.device).data_ptr()
     _lib.check(lib.mdb_conv3x3_igemm_f16(C.byref(g), _stream()), "conv3x3_igemm_f16")
     return out

@@ -276,9 +276,71 @@ def igemm_case(b, hh, ww, cin, cout, stride=1):
            flops=fl)
 
 
+SKINNY_PLANS = (("compute-bound plan", dict(skinny_ctas=0)), ("skinny plan (<= 96 CTAs)", {}),
+                 ("skinny, <= 132 CTAs", dict(skinny_ctas=132)), ("skinny, >= 4 chunks/split", dict(split_min_chunks=4)))
+
+
+def skinny_cases():
+    """The weight-bound layers of a one-frame step (the UNet pair at M = 2hw, the pose net at M = hw), each under the
+    plans of SKINNY_PLANS, alternated twice in this process.  Every one of the `reps` launches reads its own copy of the
+    weights, so they come from HBM (not from an L2 warmed by the previous launch); GB/s = weight bytes / time."""
+    reps = 20
+    cases = []
+    for m in (128, 64):  # 8x8: encoder 10-11, middle, decoder 0-2
+        cases += [(f"8x8 M={m} proj/to_out 1280x1280", m, 1280, 1280, None),
+                  (f"8x8 M={m} attn1 q|k 2560x1280", m, 2560, 1280, None),
+                  (f"8x8 M={m} ff out 1280x5120", m, 1280, 5120, None),
+                  (f"8x8 M={m} skip 1x1 1280x2560", m, 1280, 2560, None),
+                  (f"8x8 M={m} conv 1280->1280", m, 1280, 9 * 1280, (m // 64, 8, 8, 1280)),
+                  (f"8x8 M={m} conv 2560->1280", m, 1280, 9 * 2560, (m // 64, 8, 8, 2560))]
+    cases += [("8x8 attn1 V^T M=1280 N=128", 1280, 128, 1280, None),
+              ("16x16 M=512 1280x1280", 512, 1280, 1280, None), ("16x16 M=256 1280x1280", 256, 1280, 1280, None),
+              ("16x16 M=512 conv 1280->1280", 512, 1280, 9 * 1280, (2, 16, 16, 1280)),
+              ("14x8 B=2 conv 1280->1280 (im2col)", 224, 1280, 9 * 1280, (2, 14, 8, 1280))]
+    for name, m, n, k, conv in cases:
+        a = h(m, k) if conv is None else h(conv[0] * conv[1] * conv[2], conv[3])
+        ws = [h(n, k) for _ in range(reps)]
+        bias, out = f(n), torch.empty(m, n, device=D, dtype=torch.float16)
+        if conv is None:
+            run = lambda w: ops.gemm(a, w, bias=bias, out=out)
+        elif conv[1:3] == (14, 8):
+            run = lambda w: ops.conv3x3_igemm(a, w, conv=conv, bias=bias, out=out)
+        else:
+            run = lambda w: ops.gemm(a, w, bias=bias, conv=conv, out=out)
+        res = {}
+        for _ in range(2):
+            for label, kw in SKINNY_PLANS:
+                with ops.tuning(**kw):
+                    run(ws[0])
+                    torch.cuda.synchronize()
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g):
+                        for w in ws:
+                            run(w)
+                for _ in range(3):
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    g.replay()
+                    e1.record()
+                    torch.cuda.synchronize()
+                    us = e0.elapsed_time(e1) * 1e3 / reps
+                    res[label] = min(res.get(label, 1e9), us)
+                del g
+        for label, _ in SKINNY_PLANS:
+            us = res[label]
+            print(f"{name:36s} {label:28s} {us:8.2f} us  {2.0 * n * k / us / 1e3:7.1f} GB/s", flush=True)
+
+
 def main():
     which = sys.argv[1] if len(sys.argv) > 1 else "all"
     ops.ensure_device()
+    if which == "skinny":
+        import subprocess
+        smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True).stdout.strip()
+        print(f"GPU: {torch.cuda.get_device_name()} | nvidia-smi: {smi}", flush=True)
+        skinny_cases()
+        return
     if which == "igemm":
         import subprocess
         smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
