@@ -15,7 +15,8 @@ norm parameters, biases and the timestep path fp32.
 
 Weights are read from a plain state dict with the reference's key names (SURVEY §8b), repacked
 once here.  Nothing in this file computes on the CPU or through torch operators on the per-step
-path: torch only allocates buffers.
+path: torch only allocates buffers, and at levels whose token count is not a multiple of 8 copies the V^T operand's
+tokens into their padded layout (ops.pad_tokens).
 """
 from __future__ import annotations
 
@@ -297,6 +298,12 @@ def conv3x3(x: Act, w, bias, *, cout, stride=1, residual=None, bias_batch_stride
     return Act(y, x.b, ho, wo)
 
 
+def _vt(wv, x, b, out=None):
+    """(V^T = W_v x^T as [C, b*ldv], ldv): each sample's column block starts at a multiple of 8 (ops.pad_tokens)"""
+    xp, ldv = ops.pad_tokens(x, b)
+    return ops.gemm(wv, xp, out=out), ldv
+
+
 class _BankComplete(Exception):
     """unwinds appearance_write as soon as the last norm1 state is in the bank"""
 
@@ -349,13 +356,7 @@ class DenoiseEngine:
             return hit[0]
         b, n, cd = ctx16.shape
         flat = ctx16.reshape(b * n, cd)
-        ldv = (n + 7) // 8 * 8
-        # tokens padded to ldv per sample with zero rows: ONE swapped-operand GEMM then yields V^T [C, b*ldv] in the
-        # attention kernel's layout.  The kernel never reads columns n..ldv of a sample: its V^T tensor map ends
-        # each sample's keys at n and zero-fills the rest of the ragged tile
-        padded = torch.zeros((b, ldv, cd), dtype=torch.float16, device=self.device)
-        padded[:, :n].copy_(ctx16)
-        padded = padded.reshape(b * ldv, cd)
+        padded, ldv = ops.pad_tokens(flat, b)  # 77 tokens -> V^T [C, b*80]
         res = []
         for a in net.attn_layers():
             k = ops.gemm(flat, a.wk2)
@@ -413,14 +414,17 @@ class DenoiseEngine:
                 # the LAST bank entry has been produced: everything after it in the appearance net (this
                 # block's attentions and feed-forward, the rest of the decoder) is dead compute (SURVEY §8a a4)
                 raise _BankComplete()
-        vt, join_v = self._fork(lambda: ops.gemm(a.wv, n1))  # [C, B*N] == V^T
+        # V^T [C, B*ldv] from the tokens padded per sample (a copy only where n % 8 != 0, on the auxiliary stream with
+        # the GEMM); q and k stay on the unpadded rows
+        (vt, ldv), join_v = self._fork(lambda: _vt(a.wv, n1, b))
         qk = ops.gemm(n1, a.wqk)
         join_v()
         kw = {}
         if mode == "read" and bank_kv is not None:
             k1, vt1, nb1, kvb1 = bank_kv
-            kw = dict(k1=k1, vt1=vt1, n1=nb1, kv1_batches=kvb1, bank_batches=min(bank_batches, b))
-        at = ops.attention(qk[:, :c], qk[:, c:], vt, n, heads=a.heads, d=a.d, batch=b, nq=n, **kw)
+            kw = dict(k1=k1, vt1=vt1, n1=nb1, kv1_batches=kvb1, ldv1_batch=vt1.shape[1] // kvb1,
+                      bank_batches=min(bank_batches, b))
+        at = ops.attention(qk[:, :c], qk[:, c:], vt, n, heads=a.heads, d=a.d, batch=b, nq=n, ldv0_batch=ldv, **kw)
         h = ops.gemm(at, a.wo, bias=a.bo, residual=h)
         # --- attn2 (text) ---
         # norm2 is folded into the projection: W diag(gamma) on the raw h, row statistics taken by the GEMM's epilogue
@@ -512,8 +516,10 @@ class DenoiseEngine:
     def project_bank(self, bank, batches, out=None):
         """K/V of the bank under the DENOISING UNet's attn1.to_k/to_v (attention.py:289,307):
         algebraically identical to projecting cat([x_norm1] + bank) (SURVEY §8a semantics 1).
-        Returns per layer (K [batches*N, C], V^T [C, batches*N], N, batches); with `out` (a list of
-        such tuples aliasing preallocated storage, see parallel.BankLayout) the GEMMs write in place."""
+        Returns per layer (K [batches*N, C], V^T [C, batches*ldv], N, batches): each sample's V^T column block is
+        ldv = V^T.shape[1] // batches wide (N rounded up to a multiple of 8, ops.pad_tokens), the attention's
+        ldv1_batch.  With `out` (a list of such tuples aliasing preallocated storage, see parallel.BankLayout) the
+        GEMMs write in place."""
         res = []
         layers = self.unet.attn_layers()
         assert len(layers) == len(bank)
@@ -522,7 +528,7 @@ class DenoiseEngine:
             rows = n1.shape[0]
             ko, vo = (out[i][0], out[i][1]) if out is not None else (None, None)
             k1 = ops.gemm(n1, a.wqk[c:], out=ko)
-            vt1 = ops.gemm(a.wv, n1, out=vo)
+            vt1, _ = _vt(a.wv, n1, batches, out=vo)
             res.append((k1, vt1, rows // batches, batches))
         return res
 

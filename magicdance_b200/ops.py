@@ -424,6 +424,18 @@ def conv3x3_igemm_ad(x, w, *, w_param=None, bias=None, bias_batch_stride=0, rows
                               splits)
 
 
+def pad_tokens(x, b):
+    """[b*n, C] token matrix -> ([b*ldv, C], ldv) with ldv = n rounded up to a multiple of 8: zero rows after each
+    sample's tokens, so that the swapped-operand GEMM W_v x^T yields V^T [C, b*ldv] whose per-sample column blocks are
+    16-byte aligned (the attention kernels' ldv*_batch).  The kernels never read the padding columns: the V^T tensor
+    map ends each sample at n.  x itself when n % 8 == 0 (no copy, no launch); differentiable."""
+    n = x.shape[0] // b
+    ldv = (n + 7) // 8 * 8
+    if ldv == n:
+        return x, ldv
+    return torch.nn.functional.pad(x.reshape(b, n, x.shape[1]), (0, 0, 0, ldv - n)).reshape(b * ldv, -1), ldv
+
+
 def _rows8(t):
     """t as a [rows, cols] fp16 matrix whose row stride is a multiple of 8 (the kernels' alignment), copied if not"""
     if t.stride(1) == 1 and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0:

@@ -36,23 +36,30 @@ def owner_slot(indices: Sequence[int], world: int) -> Dict[int, Tuple[int, int]]
 
 
 class BankLayout:
-    """Flat fp16 layout of one timestep's bank K/V: per attention layer K [rows, C] then V^T [C, rows]."""
+    """Flat fp16 layout of one timestep's bank K/V: per attention layer K [rows, C] then V^T [C, ldv], ldv = rows
+    rounded up to a multiple of 8 (the attention kernels' V^T column alignment; the padding columns are never read).
+    Every block starts 16-byte aligned (C is a multiple of 8).  Where every layer's rows are a multiple of 8 (every
+    level of a 512x512 image) V^T is [C, rows] and the layout is unpadded."""
 
     def __init__(self, layer_shapes: Sequence[Tuple[int, int]]):
         self.layer_shapes = list(layer_shapes)  # (rows = ref_batches * N_l, C_l)
+        self.ldv = [(rows + 7) // 8 * 8 for rows, _ in self.layer_shapes]
         self.offsets = []
         off = 0
-        for rows, c in self.layer_shapes:
+        for (rows, c), ldv in zip(self.layer_shapes, self.ldv):
             self.offsets.append(off)
-            off += 2 * rows * c
+            off += rows * c + c * ldv
         self.numel = (off + 127) // 128 * 128
 
     def views(self, flat: torch.Tensor, tokens_per_batch: Sequence[int], batches: int):
-        """flat [numel] -> list of (K, V^T, N_l, batches) tuples aliasing the buffer."""
+        """flat [numel] -> list of (K, V^T, N_l, batches) tuples aliasing the buffer, V^T [C, ldv] (project_bank's
+        tuples: each sample's V^T column block is V^T.shape[1] // batches wide)."""
         res = []
-        for (rows, c), off, n in zip(self.layer_shapes, self.offsets, tokens_per_batch):
+        for (rows, c), ldv, off, n in zip(self.layer_shapes, self.ldv, self.offsets, tokens_per_batch):
+            # per-sample blocks of ldv // batches columns: one sample, or tokens already a multiple of 8
+            assert rows == n * batches and ldv == batches * ((n + 7) // 8 * 8), (rows, n, batches)
             k = flat[off:off + rows * c].view(rows, c)
-            vt = flat[off + rows * c:off + 2 * rows * c].view(c, rows)
+            vt = flat[off + rows * c:off + rows * c + c * ldv].view(c, ldv)
             res.append((k, vt, n, batches))
         return res
 

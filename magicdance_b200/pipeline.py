@@ -149,10 +149,10 @@ def build_bank_slots(eng: DenoiseEngine, ref_latent, t_vec, context, layout, tok
     tb = t_vec.shape[0]
     ref = ref_latent[:1].expand(tb, -1, -1, -1).contiguous()
     kv = eng.bank_kv(ref, t_vec, context[:1])
-    for (k, vt, n, _), (rows, c), off in zip(kv, layout.layer_shapes, layout.offsets):
-        # K [tb*n, c] -> slot j rows; V^T [c, tb*n] -> slot j [c, n]
+    for (k, vt, n, _), (rows, c), ldv, off in zip(kv, layout.layer_shapes, layout.ldv, layout.offsets):
+        # K [tb*n, c] -> slot j rows; V^T [c, tb*ldv] -> slot j [c, ldv]
         out_slots[:, off:off + n * c].view(tb, n, c).copy_(k.view(tb, n, c))
-        out_slots[:, off + n * c:off + 2 * n * c].view(tb, c, n).copy_(vt.view(c, tb, n).permute(1, 0, 2))
+        out_slots[:, off + n * c:off + n * c + c * ldv].view(tb, c, ldv).copy_(vt.view(c, tb, ldv).permute(1, 0, 2))
 
 
 def plan_bank_chunks(indices, chunk):

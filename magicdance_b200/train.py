@@ -258,19 +258,10 @@ def _conv3x3(x: Act, w, cout, *, stride=1, bias=None, residual=None, bias_batch_
     return Act(y, x.b, ho, wo)
 
 
-def _pad_tokens(x, b):
-    """[b*n, C] -> [b*ldv, C] with ldv = n rounded up to a multiple of 8 (zero rows after each sample's tokens)"""
-    n = x.shape[0] // b
-    ldv = (n + 7) // 8 * 8
-    if ldv == n:
-        return x, ldv
-    return torch.nn.functional.pad(x.reshape(b, n, x.shape[1]), (0, 0, 0, ldv - n)).reshape(b * ldv, -1), ldv
-
-
 def _vt(w, x, b):
     """V^T = W_v x^T as [C, b*ldv]: each sample's columns start at a multiple of 8 (the attention kernels' V^T
     alignment; the deepest level of a 16x16 latent has 4 tokens), the padding columns are never read"""
-    xp, ldv = _pad_tokens(x, b)
+    xp, ldv = ops.pad_tokens(x, b)
     return ops.tc_gemm(w[0], xp, a_param=w[1]), ldv
 
 
@@ -383,7 +374,7 @@ def _text(context16):
     """(context [B*77, 768], the same padded to a multiple of 8 tokens per sample [B*ldv, 768], tokens, ldv)"""
     b, nt, cd = context16.shape
     flat = context16.reshape(b * nt, cd)
-    pad, ldv = _pad_tokens(flat, b)
+    pad, ldv = ops.pad_tokens(flat, b)
     return flat, pad, nt, ldv
 
 
