@@ -210,7 +210,8 @@ int mdb_attention_lse_f16(const mdb_attn_desc* desc, float* lse, mdb_stream_t st
  *   dk0 / dk1    : fp16, laid out like k* [B*N][heads*d]           (row stride lddk*)
  *   dvt0 / dvt1  : fp16, laid out like vt* [heads*d][B*ldv_batch]  (row stride lddvt*, the forward's ldv*_batch):
  *                  only valid key columns are written; padding columns, and the bank rows / columns of batch
- *                  elements b >= bank_batches, are left as they are
+ *                  elements b >= bank_batches, are left as they are; those bank rows of k1 and columns of vt1 are
+ *                  never read, so they may hold anything, NaN and Inf included
  *   ws           : fp32 workspace of mdb_attention_bwd_ws_floats(batch, heads, nq) floats (no initial value needed)
  * Shared sources (kv*_batches == 1 with batch > 1) are rejected: their gradient needs a reduction across batch
  * elements.  Training has one bank and one prompt per sample.

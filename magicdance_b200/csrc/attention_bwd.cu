@@ -119,7 +119,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) attn_bwd_dq_kernel(const __grid
         mbar_expect_tx(&kv_full[s], C::kDqStage);
         uint8_t* sk = sKV + s * C::kDqStage;
         for (int dc = 0; dc < C::kDkChunks; ++dc)
-          tma_load_3d(sk + dc * C::kChunk64, src ? &p.tmK1 : &p.tmK0, &kv_full[s], dc * 64, head, b * p.n[src] + key0);
+          tma_load_4d(sk + dc * C::kChunk64, src ? &p.tmK1 : &p.tmK0, &kv_full[s], dc * 64, head, key0, b);
         tma_load_3d(sk + C::kTile64, src ? &p.tmV1 : &p.tmV0, &kv_full[s], key0, b, head * D);
       }
     }
@@ -269,8 +269,8 @@ __global__ void __launch_bounds__(kWsThreads, 1) attn_bwd_dkdv_kernel(const __gr
       mbar_expect_tx(&kv_bar, C::kTile128 + (kDK ? 2 * C::kVtBytes : 0));
       for (int dc = 0; dc < C::kDkChunks; ++dc)
         for (int half = 0; half < 2; ++half)
-          tma_load_3d(sK + dc * C::kChunk128 + half * C::kChunk64, src ? &p.tmK1 : &p.tmK0, &kv_bar, dc * 64, head,
-                      b * nsrc + key0 + half * kBwdStep);
+          tma_load_4d(sK + dc * C::kChunk128 + half * C::kChunk64, src ? &p.tmK1 : &p.tmK0, &kv_bar, dc * 64, head,
+                      key0 + half * kBwdStep, b);
       if (kDK)
         for (int half = 0; half < 2; ++half)
           tma_load_3d(sVt + half * C::kVtBytes, src ? &p.tmV1 : &p.tmV0, &kv_bar, key0 + half * kBwdStep, b,
@@ -433,6 +433,11 @@ static int bwd_launch(const mdb_attn_bwd_desc* a, cudaStream_t st) {
   auto mk_rows = [&](CUtensorMap* m, const void* base, long long ld, long long rows) -> int {
     return tmap_heads(m, base, D, f->heads, rows, ld, kBwdStep);
   };
+  // K per sample: keys past n are zero-filled rather than the next sample's rows.  dQ = dS K reduces over keys, and
+  // dS = 0 there does not cancel a NaN or Inf in bank rows of samples >= bank_batches, which are never read
+  auto mk_k = [&](CUtensorMap* m, const void* base, long long ld, int n, int nb) -> int {
+    return tmap_heads_per_sample(m, base, D, f->heads, n, nb, ld, kBwdStep);
+  };
   // kDV rows from row head * d: rows past d (d = 40 -> 48) are the next head's or zero-filled; they meet only the
   // zero-filled channels d..47 of the dO tile.  Keys past n are zero-filled (tmap_vt): dS = P (dP - D) is 0 there
   // only if dP is finite
@@ -441,11 +446,11 @@ static int bwd_launch(const mdb_attn_bwd_desc* a, cudaStream_t st) {
   };
   if ((rc = mk_rows(&kp.tmQ, f->q, f->ldq, (long long)f->batch * f->nq))) return rc;
   if ((rc = mk_rows(&kp.tmDO, a->dout, a->lddout, (long long)f->batch * f->nq))) return rc;
-  if ((rc = mk_rows(&kp.tmK0, f->k0, f->ldk0, (long long)f->kv0_batches * f->n0))) return rc;
+  if ((rc = mk_k(&kp.tmK0, f->k0, f->ldk0, f->n0, f->kv0_batches))) return rc;
   if ((rc = mk_vt(&kp.tmV0, f->vt0, f->ldvt0, f->n0, f->kv0_batches, f->ldv0_batch))) return rc;
   const bool bank = f->n1 > 0 && f->bank_batches > 0;
   if (bank) {
-    if ((rc = mk_rows(&kp.tmK1, f->k1, f->ldk1, (long long)f->kv1_batches * f->n1))) return rc;
+    if ((rc = mk_k(&kp.tmK1, f->k1, f->ldk1, f->n1, f->kv1_batches))) return rc;
     if ((rc = mk_vt(&kp.tmV1, f->vt1, f->ldvt1, f->n1, f->kv1_batches, f->ldv1_batch))) return rc;
   }
   kp.out = static_cast<const __half*>(f->out);

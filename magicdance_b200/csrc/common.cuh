@@ -57,6 +57,11 @@ int tmap_rows(CUtensorMap* out, const void* base, uint64_t inner, uint64_t rows,
 // 1 head x box_tokens tokens, zero-filled beyond d
 int tmap_heads(CUtensorMap* out, const void* base, int d, int heads, uint64_t tokens, long long ld,
                uint32_t box_tokens);
+// The same head slices of nb samples of n tokens each as (d, heads, token, sample); boxes of 64 channels x 1 head x
+// box_tokens tokens x 1 sample.  Tokens >= n are zero-filled, so a sample's last ragged box never reaches into the
+// next sample's rows.
+int tmap_heads_per_sample(CUtensorMap* out, const void* base, int d, int heads, int n, int nb, long long ld,
+                          uint32_t box_tokens);
 // V^T of attention: `rows` channel rows (row stride ldvt) of nb samples' column blocks of ldvb columns, the first n
 // of each used, as (key, sample, row); boxes of 64 keys x 1 sample x box_rows rows.  Keys >= n are zero-filled, so
 // the padding columns n..ldvb and the next sample's keys never reach shared memory.

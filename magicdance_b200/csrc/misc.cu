@@ -88,6 +88,14 @@ int tmap_heads(CUtensorMap* out, const void* base, int d, int heads, uint64_t to
   return make_tmap_f16(out, base, 3, dims, str, box);
 }
 
+int tmap_heads_per_sample(CUtensorMap* out, const void* base, int d, int heads, int n, int nb, long long ld,
+                          uint32_t box_tokens) {
+  const uint64_t dims[4] = {(uint64_t)d, (uint64_t)heads, (uint64_t)n, (uint64_t)nb};
+  const uint64_t str[3] = {(uint64_t)d * 2, (uint64_t)ld * 2, (uint64_t)ld * n * 2};
+  const uint32_t box[4] = {64, 1, box_tokens, 1};
+  return make_tmap_f16(out, base, 4, dims, str, box);
+}
+
 int tmap_vt(CUtensorMap* out, const void* base, int n, int nb, long long ldvb, int rows, long long ldvt,
             uint32_t box_rows) {
   const uint64_t dims[3] = {(uint64_t)n, (uint64_t)nb, (uint64_t)rows};

@@ -551,12 +551,32 @@ def attention(q, k0, vt0, n0, *, heads, d, batch, nq, out=None, kv0_batches=None
     return out
 
 
+def _attn_grad_out(t, like, name):
+    """a given out_* destination of attention_backward: fp16, 2-D, unit column stride, shaped like `like`, row stride
+    a multiple of 8"""
+    if like is None:
+        raise RuntimeError(f"magicdance_b200: {name} given without the operand it is the gradient of")
+    if t.dtype != torch.float16 or t.dim() != 2 or t.stride(1) != 1 or t.stride(0) % 8 != 0:
+        raise RuntimeError(f"magicdance_b200: {name} must be a 2-D float16 tensor with unit column stride and a row "
+                           f"stride that is a multiple of 8 (got {t.dtype}, strides {tuple(t.stride())})")
+    if tuple(t.shape) != tuple(like.shape):
+        raise RuntimeError(f"magicdance_b200: {name} must have shape {tuple(like.shape)}, got {tuple(t.shape)}")
+
+
 def attention_backward(q, k0, vt0, n0, out, dout, lse, *, heads, d, batch, nq, kv0_batches=None, ldv0_batch=None,
-                       k1=None, vt1=None, n1=0, kv1_batches=1, ldv1_batch=None, bank_batches=0, scale=None):
+                       k1=None, vt1=None, n1=0, kv1_batches=1, ldv1_batch=None, bank_batches=0, scale=None,
+                       out_dq=None, out_dk0=None, out_dvt0=None, out_dk1=None, out_dvt1=None):
     """Gradients of attention() with respect to q, k0, vt0, k1, vt1 from dout (the gradient of `out`), given the
     forward's `out` and `lse`.  Returns (dq, dk0, dvt0, dk1, dvt1) shaped like q, k0, vt0, k1, vt1 (dk1 / dvt1 are
-    None without a bank); padding columns of dvt*, and the bank rows of batch elements >= bank_batches, are zero.
+    None without a bank).  Each goes to its out_* tensor when given (fp16, 2-D, unit column stride, row stride a
+    multiple of 8); the kernels do not write the padding columns of dvt* nor the bank rows / columns of batch elements
+    >= bank_batches, which keep their contents there, and are zero in the new tensors made otherwise.
     Deterministic (csrc/attention_bwd.cu).  Shared sources (kv*_batches == 1 with batch > 1) are not supported."""
+    given = dict(out_dq=(out_dq, q), out_dk0=(out_dk0, k0), out_dvt0=(out_dvt0, vt0),
+                 out_dk1=(out_dk1, k1 if n1 > 0 else None), out_dvt1=(out_dvt1, vt1 if n1 > 0 else None))
+    for nm, (t, like) in given.items():
+        if t is not None:
+            _attn_grad_out(t, like, nm)
     lib = _lib.load()
     for t, nm in ((q, "q"), (dout, "dout")):
         _chk(t, torch.float16, nm)
@@ -568,16 +588,19 @@ def attention_backward(q, k0, vt0, n0, out, dout, lse, *, heads, d, batch, nq, k
                        ldv0_batch=ldv0_batch, k1=k1, vt1=vt1, n1=n1, kv1_batches=kv1_batches, ldv1_batch=ldv1_batch,
                        bank_batches=bank_batches, scale=scale)
     dev = q.device
-    dq = torch.empty(q.shape, dtype=torch.float16, device=dev)
-    dk0 = torch.empty(k0.shape, dtype=torch.float16, device=dev)
-    dvt0 = torch.zeros(vt0.shape, dtype=torch.float16, device=dev)
+    for nm, (t, _) in given.items():
+        if t is not None:
+            _chk(t, torch.float16, nm)
+    dq = torch.empty(q.shape, dtype=torch.float16, device=dev) if out_dq is None else out_dq
+    dk0 = torch.empty(k0.shape, dtype=torch.float16, device=dev) if out_dk0 is None else out_dk0
+    dvt0 = torch.zeros(vt0.shape, dtype=torch.float16, device=dev) if out_dvt0 is None else out_dvt0
     a.dout, a.lddout, a.lse = dout.data_ptr(), dout.stride(0), lse.data_ptr()
     a.dq, a.lddq = dq.data_ptr(), dq.stride(0)
     a.dk0, a.lddk0, a.dvt0, a.lddvt0 = dk0.data_ptr(), dk0.stride(0), dvt0.data_ptr(), dvt0.stride(0)
     dk1 = dvt1 = None
     if n1 > 0:
-        dk1 = torch.zeros(k1.shape, dtype=torch.float16, device=dev)
-        dvt1 = torch.zeros(vt1.shape, dtype=torch.float16, device=dev)
+        dk1 = torch.zeros(k1.shape, dtype=torch.float16, device=dev) if out_dk1 is None else out_dk1
+        dvt1 = torch.zeros(vt1.shape, dtype=torch.float16, device=dev) if out_dvt1 is None else out_dvt1
         a.dk1, a.lddk1, a.dvt1, a.lddvt1 = dk1.data_ptr(), dk1.stride(0), dvt1.data_ptr(), dvt1.stride(0)
     ws = _workspace("attn_bwd", int(lib.mdb_attention_bwd_ws_floats(batch, heads, nq)), torch.float32, dev)
     a.ws = ws.data_ptr()

@@ -11,6 +11,8 @@ write outside the output, nor a read of operand padding that happens to be zero.
   allocator is filled with the sentinel first.
 - `block_rel` / `gated`: rel-L2 per output block, so that an error confined to one tile is not averaged away by
   the rest.
+- `poison_workspace`: the op's scratch buffer holds the sentinel, so a read of scratch the kernel has not written
+  yet shows as NaN.
 
 CPU-only code: tests/test_kernel_edges_cpu.py checks that the checks catch what they are meant to catch."""
 import torch
@@ -22,7 +24,10 @@ SENTINEL = {torch.float16: (torch.int16, 0x7E5A), torch.float32: (torch.int32, 0
 # HBM3 (700 W power limit) over the 190 gated cases of tests/kernel_cases.py, the worst block of any case was 0.14 x
 # its tolerance (4.3e-4 against 3e-3, folded LayerNorm at M = 1); the global rel-L2 of those cases reaches 0.1 x.
 # A factor of 2 leaves that natural spread far below the gate and still fails an error confined to one tile that
-# the whole-output rel-L2 averages away.
+# the whole-output rel-L2 averages away.  On the same card, over the 178 gated backward cases (tests/gemm_bwd_cases.py,
+# attention_bwd_cases.py, norm_bwd_cases.py), the worst block was 1.17 x its tolerance (attention dq at d = 160 with
+# a near one-hot softmax, where dS = P (dP - D) cancels); outside the sharp-softmax cases the worst was 0.64 x
+# (attention, one query), and 0.2 x outside attention.
 BLOCK_FACTOR = 2.0
 
 
@@ -40,7 +45,9 @@ class Guarded:
     (row stride cols), for kernels that take a bare pointer, and `shape` reshapes it."""
 
     def __init__(self, rows, cols, dtype=torch.float16, *, contiguous=False, top=8, bottom=128, left=8, right=8,
-                 shape=None, device="cuda"):
+                 shape=None, keep=None, device="cuda"):
+        """keep: optional bool [rows, cols] mask of interior elements the kernel must NOT write (the padding columns
+        of a per-sample V^T block, the bank rows of samples without a bank); check() treats them as guard elements"""
         if contiguous:
             left, right, ld = 0, 0, cols
         else:
@@ -50,12 +57,16 @@ class Guarded:
         self.buf = poison_(torch.empty((top + rows + bottom, ld), dtype=dtype, device=device))
         self.guard = torch.ones(self.buf.shape, dtype=torch.bool, device=device)
         self.guard[top:top + rows, left:left + cols] = False
+        if keep is not None:
+            assert tuple(keep.shape) == (rows, cols)
+            self.guard[top:top + rows, left:left + cols] = keep.to(device)
         out = self.buf[top:top + rows, left:left + cols]
         self.out = out if shape is None else out.view(shape)
         assert self.out.data_ptr() % 16 == 0 and (contiguous or ld % 8 == 0)
 
     def check(self, what="output"):
-        """asserts that every interior element was written (is finite) and that no guard element was"""
+        """asserts that every interior element outside `keep` was written (is finite) and that no guard or `keep`
+        element was"""
         idt, bits = SENTINEL[self.buf.dtype]
         stray = (self.buf.view(idt) != bits) & self.guard
         if bool(stray.any()):
@@ -88,6 +99,35 @@ def check_poisoned(result, ptr, what="result"):
                                       f"{result.data_ptr():#x}, poisoned {ptr:#x}); the unwritten-element check "
                                       f"cannot run")
     check_finite(result, what)
+
+
+def bit_equal(a, b):
+    """a and b hold the same bits (torch.equal is False wherever both hold the same NaN, e.g. the sentinel an
+    output must keep)"""
+    idt = SENTINEL[a.dtype][0]
+    return a.dtype == b.dtype and a.shape == b.shape and torch.equal(a.view(idt), b.view(idt))
+
+
+def poison_workspace(key, need=0, device="cuda"):
+    """Fills the op's scratch buffer `key` (ops._workspace, grown to at least `need` fp32 elements) with the
+    sentinel and returns it, for the workspaces documented as needing no initial value ("gemm_bwd", "attn_bwd",
+    "ln_bwd"; not "gn_bwd", whose tickets must start at zero).  A kernel that reads an element before writing it
+    turns its result into NaN.  The op reuses the buffer as long as its own need is not larger;
+    check_workspace_used asserts that it did."""
+    from magicdance_b200 import ops
+    return poison_(ops._workspace(key, need, torch.float32, _op_device(device)))
+
+
+def check_workspace_used(key, buf, what="output", device="cuda"):
+    from magicdance_b200 import ops
+    cur = ops._ws_cache.get((key, _op_device(device), ops.current_lane()))
+    assert cur is buf, f"{what}: the op outgrew the poisoned {key!r} workspace; the poisoned run proves nothing"
+
+
+def _op_device(device):
+    """the device as an op's operand reports it (ops._workspace keys on tensor.device, which carries the index)"""
+    d = torch.device(device)
+    return torch.device(d.type, torch.cuda.current_device()) if d.type == "cuda" and d.index is None else d
 
 
 def rel(a, b):

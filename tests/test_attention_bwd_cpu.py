@@ -108,4 +108,43 @@ def test_backward_case_list_is_well_formed():
     from tests import attention_bwd_cases as A
     sig = inspect.signature(A.case_attention_bwd)
     for args in A.CASES:
-        sig.bind(*args)
+        sig.bind(**args) if isinstance(args, dict) else sig.bind(*args)
+    assert len({A.case_id(a) for a in A.CASES}) == len(A.CASES)
+
+
+def _cpu_operands():
+    q = torch.zeros(64, 320).half()
+    return q, dict(heads=8, d=40, batch=1, nq=64)
+
+
+@pytest.mark.parametrize("name, bad, match", [
+    ("out_dq", lambda q: torch.zeros(64, 320), "2-D float16"),                        # fp32
+    ("out_dk0", lambda q: torch.zeros(320, 64).half().t(), "unit column stride"),     # transposed
+    ("out_dk0", lambda q: torch.zeros(64, 324).half()[:, :320], "multiple of 8"),    # row stride 324
+    ("out_dvt0", lambda q: torch.zeros(320, 72).half(), "shape \\(320, 64\\)"),    # wrong width
+    ("out_dq", lambda q: torch.zeros(1, 64, 320).half(), "2-D"),
+    ("out_dk1", lambda q: torch.zeros(64, 320).half(), "without the operand"),       # no bank (n1 = 0)
+])
+def test_backward_output_buffers_are_validated_before_any_launch(name, bad, match):
+    """out_dq / out_dk0 / out_dvt0 / out_dk1 / out_dvt1 of ops.attention_backward: fp16, 2-D, unit column stride,
+    the operand's shape, a row stride that is a multiple of 8; refused with a message before the library is asked
+    to do anything, with or without a GPU"""
+    from magicdance_b200 import ops
+    q, kw = _cpu_operands()
+    n0 = ops.launch_count()
+    with pytest.raises(RuntimeError, match=match):
+        ops.attention_backward(q, q, q.t().contiguous(), 64, q, q, torch.zeros(1, 8, 64), **kw, **{name: bad(q)})
+    assert ops.launch_count() == n0
+
+
+def test_backward_takes_valid_output_buffers_up_to_the_device_check():
+    """well-formed out_* buffers (a row stride wider than the row) pass the validation; on a machine without a GPU
+    the call then stops at the CUDA-tensor check"""
+    from magicdance_b200 import ops
+    if torch.cuda.is_available():
+        pytest.skip("GPU present")
+    q, kw = _cpu_operands()
+    outs = dict(out_dq=torch.zeros(64, 336).half()[:, :320], out_dk0=torch.zeros(64, 320).half(),
+                out_dvt0=torch.zeros(320, 64).half())
+    with pytest.raises(RuntimeError, match="no CPU fallback"):
+        ops.attention_backward(q, q, q.t().contiguous(), 64, q, q, torch.zeros(1, 8, 64), **kw, **outs)

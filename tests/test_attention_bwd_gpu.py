@@ -15,10 +15,11 @@ SHAPES = [  # (batch, heads, d, nq, n0, n1, bank_batches, ldv_pad)
 ]
 
 
-@pytest.mark.parametrize("args", A.CASES, ids=["-".join(map(str, a)) for a in A.CASES])
+@pytest.mark.parametrize("args", A.CASES, ids=[A.case_id(a) for a in A.CASES])
 def test_backward_matches_torch_fp32(args):
-    err, tol, desc = A.case_attention_bwd(*args)
+    err, tol, desc = A.run_case(args)
     torch.cuda.synchronize()
+    print(desc)
     assert err <= tol, f"{desc}: error {err:.3e} > {tol:.1e}"
 
 

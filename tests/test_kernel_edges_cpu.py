@@ -102,3 +102,67 @@ def test_attention_rejects_unaligned_bank_sample_stride_before_any_launch():
         assert lib.mdb_attention_f16(C.byref(a), None) == -1
         assert "ldv1_batch must be >= n1 and % 8" in lib.mdb_last_error().decode()
     assert lib.mdb_launch_count() == n0
+
+
+def _vt_with_keep(n=77, ldv=80, batch=2, rows=40):
+    """a dvt-like Guarded [rows, batch*ldv] whose padding columns n..ldv of each sample must not be written"""
+    keep = torch.zeros(rows, batch * ldv, dtype=torch.bool)
+    for b in range(batch):
+        keep[:, b * ldv + n:(b + 1) * ldv] = True
+    gb = KG.Guarded(rows, batch * ldv, keep=keep, device="cpu")
+    for b in range(batch):
+        gb.out[:, b * ldv:b * ldv + n] = torch.randn(rows, n).half()
+    return gb
+
+
+def test_keep_mask_passes_when_only_the_allowed_elements_are_written():
+    gb = _vt_with_keep()
+    gb.check()
+    assert torch.isnan(gb.out[:, 77:80]).all()  # the keep-out columns still hold the sentinel
+
+
+def test_keep_mask_catches_a_single_write_into_a_keep_out_column():
+    gb = _vt_with_keep()
+    gb.out[5, 80 + 78] = 0.0  # sample 1's padding column 78
+    with pytest.raises(AssertionError, match="1 guard elements overwritten, the first at buffer row 13 column 166"):
+        gb.check()
+
+
+def test_keep_mask_catches_a_single_unwritten_element():
+    gb = _vt_with_keep()
+    KG.poison_(gb.out[39, 80 + 76:80 + 77])  # sample 1's last key of the last row
+    with pytest.raises(AssertionError, match="1 of 6160 elements not finite"):
+        gb.check()
+
+
+def test_keep_mask_covers_whole_rows():
+    """the bank rows of samples >= bank_batches (dk1)"""
+    keep = torch.zeros(200, 320, dtype=torch.bool)
+    keep[100:] = True
+    gb = KG.Guarded(200, 320, keep=keep, device="cpu")
+    gb.out[:100] = 1.0
+    gb.check()
+    gb.out[150, 7] = 1.0
+    with pytest.raises(AssertionError, match="1 guard elements overwritten"):
+        gb.check()
+
+
+def test_poisoned_workspace_is_the_one_the_op_gets():
+    from magicdance_b200 import ops
+    key = "kernel_guard_selftest"
+    ws = KG.poison_workspace(key, 100, device="cpu")
+    assert ws.numel() >= 100 and bool((ws.view(torch.int32) == KG.SENTINEL[torch.float32][1]).all())
+    assert ops._workspace(key, 50, torch.float32, torch.device("cpu")) is ws
+    KG.check_workspace_used(key, ws, device="cpu")
+    ops._workspace(key, 10 * ws.numel(), torch.float32, torch.device("cpu"))  # an op that needs more regrows it
+    with pytest.raises(AssertionError, match="outgrew the poisoned"):
+        KG.check_workspace_used(key, ws, device="cpu")
+    ops._ws_cache.pop((key, torch.device("cpu"), ops.current_lane()))
+
+
+def test_bit_equal_compares_nan_payloads():
+    a = KG.poison_(torch.empty(4, 8).half())
+    b = a.clone()
+    assert not torch.equal(a, b) and KG.bit_equal(a, b)
+    b[0, 0] = float("nan")  # a canonical NaN is not the sentinel
+    assert not KG.bit_equal(a, b)

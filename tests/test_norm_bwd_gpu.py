@@ -183,3 +183,28 @@ def _spatial_transformer():
         assert p[k].grad.shape == r[k].grad.shape and p[k].grad.dtype == torch.float32, k
         errs[k] = rel(p[k].grad, r[k].grad)
     _check(errs)
+
+
+def test_groupnorm_backward_calls_of_different_shapes_share_one_workspace():
+    """the statistics kernel's tickets reset themselves: a big, a small and again the big call on one "gn_bwd"
+    workspace give the bits of the same calls on fresh, zeroed workspaces (their own scratch lanes)"""
+    from magicdance_b200 import ops
+    shapes = [dict(batch=4, hw=1024, c1=640, c2=320), dict(batch=1, hw=15, c1=2560),
+              dict(batch=4, hw=1024, c1=640, c2=320)]
+
+    def call(batch, hw, c1, c2=0, seed=0):
+        x1 = _rand(batch * hw, c1, seed=seed).half()
+        x2 = _rand(batch * hw, c2, seed=seed + 1).half() if c2 else None
+        g, b = _rand(c1 + c2, seed=seed + 2).float(), _rand(c1 + c2, seed=seed + 3).float()
+        dy = _rand(batch * hw, c1 + c2, seed=seed + 4).half()
+        return ops.groupnorm_backward(x1, g, b, dy, batch=batch, hw=hw, eps=1e-5, silu=True, x2=x2)
+
+    shared = [call(**s, seed=i) for i, s in enumerate(shapes)]
+    fresh = []
+    for i, s in enumerate(shapes):
+        with ops.workspace_lane(("gn_bwd_fresh", i)):
+            fresh.append(call(**s, seed=i))
+    torch.cuda.synchronize()
+    for i, (a, b) in enumerate(zip(shared, fresh)):
+        for x, y in zip(a, b):
+            assert (x is None and y is None) or torch.equal(x, y), f"call {i} ({shapes[i]})"
