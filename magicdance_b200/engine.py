@@ -99,9 +99,8 @@ def _f32(t, device):
 
 
 def pack_conv3x3(w, device):
-    """Conv2d OIHW fp32 -> [O][kh][kw][I] fp16 viewed as [O, 9*I] (K order = tap-major, channel-minor)."""
-    o, i, kh, kw = w.shape
-    return _f16(w.detach().to(device).permute(0, 2, 3, 1).reshape(o, kh * kw * i), device)
+    """Conv2d OIHW fp32 -> [O][kh][kw][I] fp16 viewed as [O, 9*I] on `device` (ops.pack_conv_weight)."""
+    return ops.pack_conv_weight(w.detach().to(device))
 
 
 def pack_conv1x1(w, device):

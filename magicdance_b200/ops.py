@@ -6,6 +6,7 @@ below launches OUR kernels through ctypes.  No function has a PyTorch/CPU fallba
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 
 import torch
@@ -152,6 +153,32 @@ def _fill_fwd_desc(g, a, w, a2, conv, conv_stride, m):
     return m, g.k1
 
 
+def _fill_epilogue(g, w, out, n_out, device, bias, bias_batch_stride, rows_per_batch, residual, splits):
+    """fills the B operand and the epilogue fields (out, bias or per-batch bias, residual, split count and split-K
+    workspace) of the forward GemmDesc g whose A side is filled; returns out, a new [m, n_out] tensor when None"""
+    m = g.m
+    if out is None:
+        out = torch.empty((m, n_out), dtype=torch.float16, device=device)
+    _chk(out, torch.float16, "out")
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape[0] >= m and out.shape[1] == n_out, (out.shape, m, n_out)
+    assert w.stride(1) == 1
+    g.b, g.ldb = w.data_ptr(), w.stride(0)
+    g.d, g.ldd = out.data_ptr(), out.stride(0)
+    if bias is not None:
+        _chk(bias, torch.float32, "bias")
+        g.bias, g.bias_batch_stride, g.rows_per_batch = bias.data_ptr(), bias_batch_stride, rows_per_batch
+    if residual is not None:
+        _chk(residual, torch.float16, "residual")
+        assert residual.dim() == 2 and residual.stride(1) == 1
+        g.residual, g.ldr = residual.data_ptr(), residual.stride(0)
+    g.splits = splits
+    if splits > 8:
+        # the library rounds the count so that no split is empty (12 splits of 20 K chunks run as 10); up to 8 splits
+        # reduce inside a cluster, more through this workspace
+        g.splitk_ws = _workspace("splitk", splits * m * g.n, torch.float32, device).data_ptr()
+    return out
+
+
 def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, residual=None, epilogue=EPI_NONE,
          a2=None, conv=None, conv_stride=1, splits=0, m=None, ln_u=None, ln_eps=1e-5):
     """D = epilogue(A @ W^T).  a: [M, K1] fp16 (last dim contiguous, row stride arbitrary) or, with
@@ -166,37 +193,16 @@ def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, re
     g = _lib.GemmDesc()
     n, k = w.shape
     m, _ = _fill_fwd_desc(g, a, w, a2, conv, conv_stride, m)
-    n_out = n // 2 if epilogue == EPI_GEGLU else n
-    if out is None:
-        out = torch.empty((m, n_out), dtype=torch.float16, device=a.device)
-    _chk(out, torch.float16, "out")
-    assert out.dim() == 2 and out.stride(1) == 1 and out.shape[0] >= m and out.shape[1] == n_out, (out.shape, m, n_out)
-    assert w.stride(1) == 1
-    g.b, g.ldb = w.data_ptr(), w.stride(0)
-    g.d, g.ldd = out.data_ptr(), out.stride(0)
-    if bias is not None:
-        _chk(bias, torch.float32, "bias")
-        g.bias, g.bias_batch_stride, g.rows_per_batch = bias.data_ptr(), bias_batch_stride, rows_per_batch
-    if residual is not None:
-        _chk(residual, torch.float16, "residual")
-        assert residual.dim() == 2 and residual.stride(1) == 1
-        g.residual, g.ldr = residual.data_ptr(), residual.stride(0)
+    out = _fill_epilogue(g, w, out, n // 2 if epilogue == EPI_GEGLU else n, a.device, bias, bias_batch_stride,
+                         rows_per_batch, residual, 1 if ln_u is not None else splits)  # the folded LayerNorm: no split
     g.epilogue = epilogue
     if ln_u is not None:
         _chk(ln_u, torch.float32, "ln_u")
         assert conv is None and a2 is None and ln_u.numel() == n and ln_u.is_contiguous()
         g.ln_u, g.ln_eps = ln_u.data_ptr(), float(ln_eps)
-        splits = 1
     if TRACE is not None:
-        TRACE.append((m, n, k, (tuple(conv) + (conv_stride,)) if conv is not None else None, epilogue, splits,
+        TRACE.append((m, n, k, (tuple(conv) + (conv_stride,)) if conv is not None else None, epilogue, g.splits,
                       a2.shape[1] if a2 is not None else 0))
-    if splits > 8:
-        # the library rounds the count so that no split is empty (12 splits of 20 K chunks run as 10); up to 8 splits
-        # reduce inside a cluster, more through this workspace
-        ws = _workspace("splitk", splits * m * n, torch.float32, a.device)
-        g.splits, g.splitk_ws = splits, ws.data_ptr()
-    else:
-        g.splits = splits
     if _GEMM_DEBUG:  # MDB_GEMM_DEBUG=1: name every GEMM before it runs and wait for it (pins down a hanging shape)
         import sys
         print(f"gemm m={m} n={n} k={k} conv={conv} epi={epilogue} splits={g.splits} a2={a2 is not None} lda={g.lda} "
@@ -211,15 +217,101 @@ def gemm(a, w, *, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0, re
 _DTYPES = {torch.float16: 0, torch.float32: 1}  # MDB_DTYPE_F16 / MDB_DTYPE_F32
 
 
-def _grad_out(t, shape, dtype, device, name):
-    """the destination of one gradient: `t` (2-D, unit column stride) or a new tensor"""
+def _dest(t, shape, dtype, device, name, *, any_float=False, contiguous=False, rows8=False, numel=False, zero=False):
+    """The destination of one gradient: a new tensor of `shape` and `dtype` (zero-filled with zero) when the caller
+    gave none, else the caller's out_* tensor t, checked before any kernel writes through it.  t must be of dtype
+    (float16 or float32 with any_float: the gradient then takes t's dtype), dense with contiguous, else 2-D with unit
+    column stride (and with rows8 a row stride that is a multiple of 8), and of `shape` (with numel: of as many
+    elements, in any shape)."""
     if t is None:
-        t = torch.empty(shape, dtype=dtype, device=device)
-    if t.dtype not in _DTYPES:
-        raise RuntimeError(f"magicdance_b200: {name} must be float16 or float32, got {t.dtype}")
+        return (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=device)
+    dtypes = tuple(_DTYPES) if any_float else (dtype,)
+    kind = " or ".join(str(d).removeprefix("torch.") for d in dtypes)
+    if contiguous:
+        ok, want = t.is_contiguous(), f"a contiguous {kind} tensor"
+    else:
+        ok = t.dim() == 2 and t.stride(1) == 1 and (not rows8 or t.stride(0) % 8 == 0)
+        want = f"a 2-D {kind} tensor with unit column stride" + (" and a row stride that is a multiple of 8" if rows8
+                                                                  else "")
+    if t.dtype not in dtypes or not ok:
+        raise RuntimeError(f"magicdance_b200: {name} must be {want} (got {t.dtype}, strides {tuple(t.stride())})")
+    if (t.numel() != math.prod(shape)) if numel else (tuple(t.shape) != tuple(shape)):
+        want = f"{math.prod(shape)} elements" if numel else f"shape {tuple(shape)}"
+        raise RuntimeError(f"magicdance_b200: {name} must have {want}, got {tuple(t.shape)}")
     _chk(t, t.dtype, name)
-    assert t.dim() == 2 and t.stride(1) == 1 and tuple(t.shape) == tuple(shape), (name, t.shape, shape)
     return t
+
+
+def _bwd_ws(desc, ws_floats, key, device, what, zero=False):
+    """the scratch pointer of a backward descriptor: ws_floats(desc) fp32 elements of the `key` workspace (a negative
+    answer is the library's argument error, raised as `what`'s)"""
+    need = int(ws_floats(C.byref(desc)))
+    if need < 0:
+        _lib.check(need, what)
+    return _workspace(key, need, torch.float32, device, zero=zero).data_ptr()
+
+
+def _wanted(ctx, **inputs):
+    """the `grads` names of a backward wrapper that autograd needs: each name maps to the positions of the forward's
+    inputs that receive that gradient"""
+    need = ctx.needs_input_grad
+    return [nm for nm, pos in inputs.items() if any(need[i] for i in pos)]
+
+
+def pack_conv_weight(w):
+    """Conv2d weight OIHW -> the fp16 copy the kernels read: [O][kh][kw][I] as [O, kh*kw*I] (K order tap-major,
+    channel-minor)"""
+    return w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1).to(torch.float16).contiguous()
+
+
+def unpack_conv_weight(w, like):
+    """pack_conv_weight's layout undone as a view: w [O, kh*kw*I] in the layout of `like` (a Conv2d weight OIHW; a
+    matrix such as a Linear weight keeps w's own layout)"""
+    if like.dim() != 4:
+        return w.view(like.shape)
+    o, i, kh, kw = like.shape
+    return w.view(o, kh, kw, i).permute(0, 3, 1, 2)
+
+
+def _route_grad(g, operand, param):
+    """(operand's gradient, param's gradient) from g, the gradient in the kernel's layout: it goes to the fp32
+    parameter param, in param's layout, when the fp16 operand was packed from one, else to the operand"""
+    if g is None:
+        return None, None
+    if param is not None:
+        return None, unpack_conv_weight(g, param)
+    return g.view(operand.shape).to(operand.dtype), None
+
+
+def _fill_gemm_grads(g, w, dd, da_shape, da2_shape, device, ws_floats, what, *, bias_batch_stride, rows_per_batch,
+                     splits, db_splits, grads, da_dtype, db_dtype, out_da, out_da2, out_db, out_dbias, accumulate):
+    """fills the B operand, dD, the split counts, the gradient destinations (dA, and dA2 of da2_shape unless None; dB;
+    dbias) with their accumulate flags, and the workspace of the GemmBwdDesc g whose A side is filled, in
+    gemm_backward()'s conventions; returns (da, da2, dw, dbias)"""
+    f, m = g.fwd, g.fwd.m
+    n, k = w.shape
+    assert w.stride(1) == 1 and dd.shape[0] >= m and dd.shape[1] == n, (dd.shape, m, n)
+    f.b, f.ldb = w.data_ptr(), w.stride(0)
+    f.splits, f.bias_batch_stride, f.rows_per_batch = splits, bias_batch_stride, rows_per_batch
+    g.dd, g.lddd, g.splits = dd.data_ptr(), dd.stride(0), db_splits
+    acc = set(accumulate)
+    da = da2 = dw = dbias = None
+    if "a" in grads:
+        da = _dest(out_da, da_shape, da_dtype, device, "out_da", any_float=True)
+        g.da, g.ldda, g.da_dtype, g.da_accumulate = da.data_ptr(), da.stride(0), _DTYPES[da.dtype], "a" in acc
+        if da2_shape is not None:
+            da2 = _dest(out_da2, da2_shape, da_dtype, device, "out_da2", any_float=True)
+            g.da2, g.ldda2, g.da2_dtype = da2.data_ptr(), da2.stride(0), _DTYPES[da2.dtype]
+            g.da2_accumulate = "a2" in acc
+    if "b" in grads:
+        dw = _dest(out_db, (n, k), db_dtype, device, "out_db", any_float=True)
+        g.db, g.lddb, g.db_dtype, g.db_accumulate = dw.data_ptr(), dw.stride(0), _DTYPES[dw.dtype], "b" in acc
+    if "bias" in grads:
+        shape = (n,) if bias_batch_stride == 0 else (-(-m // rows_per_batch), bias_batch_stride)
+        dbias = _dest(out_dbias, shape, torch.float32, device, "out_dbias", contiguous=True)
+        g.dbias, g.dbias_accumulate = dbias.data_ptr(), "bias" in acc
+    g.ws = _bwd_ws(g, ws_floats, "gemm_bwd", device, what)
+    return da, da2, dw, dbias
 
 
 def gemm_backward(a, w, dd, *, a2=None, conv=None, conv_stride=1, bias_batch_stride=0, rows_per_batch=0, splits=0,
@@ -238,48 +330,24 @@ def gemm_backward(a, w, dd, *, a2=None, conv=None, conv_stride=1, bias_batch_str
     _chk(w, torch.float16, "w")
     _chk(dd, torch.float16, "dd")
     assert dd.dim() == 2 and dd.stride(1) == 1
-    dev = a.device
     g = _lib.GemmBwdDesc()
-    f = g.fwd
-    n, k = w.shape
-    m, k1 = _fill_fwd_desc(f, a, w, a2, conv, conv_stride, m)
-    da_shape = (conv[0] * conv[1] * conv[2], conv[3]) if conv is not None else (m, k1)
-    assert w.stride(1) == 1 and dd.shape[0] >= m and dd.shape[1] == n, (dd.shape, m, n)
-    f.b, f.ldb = w.data_ptr(), w.stride(0)
-    f.epilogue, f.splits = epilogue, splits
-    f.bias_batch_stride, f.rows_per_batch = bias_batch_stride, rows_per_batch
+    m, k1 = _fill_fwd_desc(g.fwd, a, w, a2, conv, conv_stride, m)
+    g.fwd.epilogue = epilogue
     if ln_u is not None:
-        f.ln_u = ln_u.data_ptr()
-    g.dd, g.lddd, g.splits = dd.data_ptr(), dd.stride(0), db_splits
-    acc = set(accumulate)
-    da = da2 = dw = dbias = None
-    if "a" in grads:
-        da = _grad_out(out_da, da_shape, da_dtype, dev, "out_da")
-        g.da, g.ldda, g.da_dtype, g.da_accumulate = da.data_ptr(), da.stride(0), _DTYPES[da.dtype], "a" in acc
-        if a2 is not None:
-            da2 = _grad_out(out_da2, (m, k - k1), da_dtype, dev, "out_da2")
-            g.da2, g.ldda2, g.da2_dtype = da2.data_ptr(), da2.stride(0), _DTYPES[da2.dtype]
-            g.da2_accumulate = "a2" in acc
-    if "b" in grads:
-        dw = _grad_out(out_db, (n, k), db_dtype, dev, "out_db")
-        g.db, g.lddb, g.db_dtype, g.db_accumulate = dw.data_ptr(), dw.stride(0), _DTYPES[dw.dtype], "b" in acc
-    if "bias" in grads:
-        shape = (n,) if bias_batch_stride == 0 else (-(-m // rows_per_batch), bias_batch_stride)
-        dbias = torch.empty(shape, dtype=torch.float32, device=dev) if out_dbias is None else out_dbias
-        _chk(dbias, torch.float32, "out_dbias")
-        assert dbias.is_contiguous() and tuple(dbias.shape) == shape, (dbias.shape, shape)
-        g.dbias, g.dbias_accumulate = dbias.data_ptr(), "bias" in acc
-    need = int(lib.mdb_gemm_bwd_ws_floats(C.byref(g)))
-    if need < 0:
-        _lib.check(need, "gemm_bwd_f16")
-    g.ws = _workspace("gemm_bwd", need, torch.float32, dev).data_ptr()
+        g.fwd.ln_u = ln_u.data_ptr()
+    da_shape = (conv[0] * conv[1] * conv[2], conv[3]) if conv is not None else (m, k1)
+    res = _fill_gemm_grads(g, w, dd, da_shape, (m, w.shape[1] - k1) if a2 is not None else None, a.device,
+                           lib.mdb_gemm_bwd_ws_floats, "gemm_bwd_f16", bias_batch_stride=bias_batch_stride,
+                           rows_per_batch=rows_per_batch, splits=splits, db_splits=db_splits, grads=grads,
+                           da_dtype=da_dtype, db_dtype=db_dtype, out_da=out_da, out_da2=out_da2, out_db=out_db,
+                           out_dbias=out_dbias, accumulate=accumulate)
     _lib.check(lib.mdb_gemm_bwd_f16(C.byref(g), _stream()), "gemm_bwd_f16")
-    return da, da2, dw, dbias
+    return res
 
 
 def _fill_igemm_desc(g, x, w, x2, conv, conv_stride):
     """the A-side fields and m, n, k of a GemmDesc for mdb_conv3x3_igemm_*: x [nb*h*w, k1] (x2 [nb*h*w, c - k1]) with
-    unit channel stride, any pixel stride; returns m"""
+    unit channel stride, any pixel stride"""
     nb, h, wd, c = conv
     n, k = w.shape
     assert conv_stride in (1, 2) and k == 9 * c, (conv, w.shape)
@@ -293,9 +361,7 @@ def _fill_igemm_desc(g, x, w, x2, conv, conv_stride):
     else:
         assert x.shape[1] == c, (x.shape, conv)
         g.k1 = c
-    m = _gemm_m(x, conv, conv_stride, None)
-    g.m, g.n, g.k = m, n, k
-    return m
+    g.m, g.n, g.k = _gemm_m(x, conv, conv_stride, None), n, k
 
 
 def conv3x3_igemm(x, w, *, conv, conv_stride=1, x2=None, out=None, bias=None, bias_batch_stride=0, rows_per_batch=0,
@@ -308,25 +374,8 @@ def conv3x3_igemm(x, w, *, conv, conv_stride=1, x2=None, out=None, bias=None, bi
     _chk(x, torch.float16, "x")
     _chk(w, torch.float16, "w")
     g = _lib.GemmDesc()
-    n = w.shape[0]
-    m = _fill_igemm_desc(g, x, w, x2, conv, conv_stride)
-    if out is None:
-        out = torch.empty((m, n), dtype=torch.float16, device=x.device)
-    _chk(out, torch.float16, "out")
-    assert out.dim() == 2 and out.stride(1) == 1 and out.shape[0] >= m and out.shape[1] == n, (out.shape, m, n)
-    assert w.stride(1) == 1
-    g.b, g.ldb = w.data_ptr(), w.stride(0)
-    g.d, g.ldd = out.data_ptr(), out.stride(0)
-    if bias is not None:
-        _chk(bias, torch.float32, "bias")
-        g.bias, g.bias_batch_stride, g.rows_per_batch = bias.data_ptr(), bias_batch_stride, rows_per_batch
-    if residual is not None:
-        _chk(residual, torch.float16, "residual")
-        assert residual.dim() == 2 and residual.stride(1) == 1
-        g.residual, g.ldr = residual.data_ptr(), residual.stride(0)
-    g.splits = splits
-    if splits > 8:
-        g.splitk_ws = _workspace("splitk", splits * m * n, torch.float32, x.device).data_ptr()
+    _fill_igemm_desc(g, x, w, x2, conv, conv_stride)
+    out = _fill_epilogue(g, w, out, w.shape[0], x.device, bias, bias_batch_stride, rows_per_batch, residual, splits)
     _lib.check(lib.mdb_conv3x3_igemm_f16(C.byref(g), _stream()), "conv3x3_igemm_f16")
     return out
 
@@ -341,40 +390,15 @@ def conv3x3_igemm_backward(x, w, dd, *, conv, conv_stride=1, x2=None, bias_batch
     _chk(w, torch.float16, "w")
     _chk(dd, torch.float16, "dd")
     assert dd.dim() == 2 and dd.stride(1) == 1
-    dev = x.device
     g = _lib.GemmBwdDesc()
-    f = g.fwd
-    n, k = w.shape
-    m = _fill_igemm_desc(f, x, w, x2, conv, conv_stride)
-    assert w.stride(1) == 1 and dd.shape[0] >= m and dd.shape[1] == n, (dd.shape, m, n)
-    f.b, f.ldb = w.data_ptr(), w.stride(0)
-    f.splits = splits
-    f.bias_batch_stride, f.rows_per_batch = bias_batch_stride, rows_per_batch
-    g.dd, g.lddd, g.splits = dd.data_ptr(), dd.stride(0), db_splits
-    acc = set(accumulate)
-    da = da2 = dw = dbias = None
-    if "a" in grads:
-        da = _grad_out(out_da, tuple(x.shape), da_dtype, dev, "out_da")
-        g.da, g.ldda, g.da_dtype, g.da_accumulate = da.data_ptr(), da.stride(0), _DTYPES[da.dtype], "a" in acc
-        if x2 is not None:
-            da2 = _grad_out(out_da2, tuple(x2.shape), da_dtype, dev, "out_da2")
-            g.da2, g.ldda2, g.da2_dtype = da2.data_ptr(), da2.stride(0), _DTYPES[da2.dtype]
-            g.da2_accumulate = "a2" in acc
-    if "b" in grads:
-        dw = _grad_out(out_db, (n, k), db_dtype, dev, "out_db")
-        g.db, g.lddb, g.db_dtype, g.db_accumulate = dw.data_ptr(), dw.stride(0), _DTYPES[dw.dtype], "b" in acc
-    if "bias" in grads:
-        shape = (n,) if bias_batch_stride == 0 else (-(-m // rows_per_batch), bias_batch_stride)
-        dbias = torch.empty(shape, dtype=torch.float32, device=dev) if out_dbias is None else out_dbias
-        _chk(dbias, torch.float32, "out_dbias")
-        assert dbias.is_contiguous() and tuple(dbias.shape) == shape, (dbias.shape, shape)
-        g.dbias, g.dbias_accumulate = dbias.data_ptr(), "bias" in acc
-    need = int(lib.mdb_conv3x3_igemm_bwd_ws_floats(C.byref(g)))
-    if need < 0:
-        _lib.check(need, "conv3x3_igemm_bwd_f16")
-    g.ws = _workspace("gemm_bwd", need, torch.float32, dev).data_ptr()
+    _fill_igemm_desc(g.fwd, x, w, x2, conv, conv_stride)
+    res = _fill_gemm_grads(g, w, dd, tuple(x.shape), tuple(x2.shape) if x2 is not None else None, x.device,
+                           lib.mdb_conv3x3_igemm_bwd_ws_floats, "conv3x3_igemm_bwd_f16",
+                           bias_batch_stride=bias_batch_stride, rows_per_batch=rows_per_batch, splits=splits,
+                           db_splits=db_splits, grads=grads, da_dtype=da_dtype, db_dtype=db_dtype, out_da=out_da,
+                           out_da2=out_da2, out_db=out_db, out_dbias=out_dbias, accumulate=accumulate)
     _lib.check(lib.mdb_conv3x3_igemm_bwd_f16(C.byref(g), _stream()), "conv3x3_igemm_bwd_f16")
-    return da, da2, dw, dbias
+    return res
 
 
 class Conv3x3Igemm(torch.autograd.Function):
@@ -401,16 +425,10 @@ class Conv3x3Igemm(torch.autograd.Function):
     def backward(ctx, dout):
         x, w, w_param, x2 = ctx.saved_tensors
         dd = _rows8(dout)
-        need = ctx.needs_input_grad
-        grads = [nm for nm, want in (("a", need[0] or need[5]), ("b", need[1] or need[2]), ("bias", need[3])) if want]
+        grads = _wanted(ctx, a=(0, 5), b=(1, 2), bias=(3,))
         dx, dx2, dw, dbias = conv3x3_igemm_backward(
             x, w, dd, x2=x2, grads=grads, db_dtype=torch.float32 if w_param is not None else torch.float16, **ctx.kw)
-        g_w = g_wp = None
-        if dw is not None:
-            if w_param is not None:  # Conv2d OIHW: the kernel's [O][kh][kw][I] rows, viewed
-                g_wp = dw.view(w_param.shape[0], 3, 3, -1).permute(0, 3, 1, 2)
-            else:
-                g_w = dw
+        g_w, g_wp = _route_grad(dw, w, w_param)
         g_bias = dbias.view(ctx.bias_shape) if dbias is not None else None
         g_res = dout if ctx.has_residual else None
         return dx, g_w, g_wp, g_bias, g_res, dx2, None, None, None, None, None
@@ -470,24 +488,12 @@ class TcGemm(torch.autograd.Function):
     def backward(ctx, dout):
         a, a_param, w, w_param, a2 = ctx.saved_tensors
         dd = _rows8(dout)
-        need = ctx.needs_input_grad
-        grads = [nm for nm, want in (("a", need[0] or need[1] or need[6]), ("b", need[2] or need[3]),
-                                     ("bias", need[4])) if want]
+        grads = _wanted(ctx, a=(0, 1, 6), b=(2, 3), bias=(4,))
         da, da2, dw, dbias = gemm_backward(
             a, w, dd, a2=a2, grads=grads, da_dtype=torch.float32 if a_param is not None else torch.float16,
             db_dtype=torch.float32 if w_param is not None else torch.float16, **ctx.kw)
-        g_a = g_ap = g_w = g_wp = None
-        if da is not None:
-            if a_param is not None:
-                g_ap = da.view(a_param.shape)
-            else:
-                g_a = da.view(a.shape)
-        if dw is not None:
-            if w_param is not None:
-                # Conv2d OIHW: the kernel's [O][kh][kw][I] rows, viewed
-                g_wp = dw.view(w_param.shape[0], 3, 3, -1).permute(0, 3, 1, 2) if w_param.dim() == 4 else dw
-            else:
-                g_w = dw
+        g_a, g_ap = _route_grad(da, a, a_param)
+        g_w, g_wp = _route_grad(dw, w, w_param)
         g_bias = dbias.view(ctx.bias_shape) if dbias is not None else None
         g_res = dout if ctx.has_residual else None
         return g_a, g_ap, g_w, g_wp, g_bias, g_res, da2, None, None, None, None, None, None
@@ -551,18 +557,6 @@ def attention(q, k0, vt0, n0, *, heads, d, batch, nq, out=None, kv0_batches=None
     return out
 
 
-def _attn_grad_out(t, like, name):
-    """a given out_* destination of attention_backward: fp16, 2-D, unit column stride, shaped like `like`, row stride
-    a multiple of 8"""
-    if like is None:
-        raise RuntimeError(f"magicdance_b200: {name} given without the operand it is the gradient of")
-    if t.dtype != torch.float16 or t.dim() != 2 or t.stride(1) != 1 or t.stride(0) % 8 != 0:
-        raise RuntimeError(f"magicdance_b200: {name} must be a 2-D float16 tensor with unit column stride and a row "
-                           f"stride that is a multiple of 8 (got {t.dtype}, strides {tuple(t.stride())})")
-    if tuple(t.shape) != tuple(like.shape):
-        raise RuntimeError(f"magicdance_b200: {name} must have shape {tuple(like.shape)}, got {tuple(t.shape)}")
-
-
 def attention_backward(q, k0, vt0, n0, out, dout, lse, *, heads, d, batch, nq, kv0_batches=None, ldv0_batch=None,
                        k1=None, vt1=None, n1=0, kv1_batches=1, ldv1_batch=None, bank_batches=0, scale=None,
                        out_dq=None, out_dk0=None, out_dvt0=None, out_dk1=None, out_dvt1=None):
@@ -572,11 +566,15 @@ def attention_backward(q, k0, vt0, n0, out, dout, lse, *, heads, d, batch, nq, k
     multiple of 8); the kernels do not write the padding columns of dvt* nor the bank rows / columns of batch elements
     >= bank_batches, which keep their contents there, and are zero in the new tensors made otherwise.
     Deterministic (csrc/attention_bwd.cu).  Shared sources (kv*_batches == 1 with batch > 1) are not supported."""
-    given = dict(out_dq=(out_dq, q), out_dk0=(out_dk0, k0), out_dvt0=(out_dvt0, vt0),
-                 out_dk1=(out_dk1, k1 if n1 > 0 else None), out_dvt1=(out_dvt1, vt1 if n1 > 0 else None))
-    for nm, (t, like) in given.items():
-        if t is not None:
-            _attn_grad_out(t, like, nm)
+    dests = []  # the kernels leave padding columns and unused bank rows unwritten: zeros in the new tensors
+    for nm, t, like, zero in (("out_dq", out_dq, q, False), ("out_dk0", out_dk0, k0, False),
+                              ("out_dvt0", out_dvt0, vt0, True), ("out_dk1", out_dk1, k1 if n1 > 0 else None, True),
+                              ("out_dvt1", out_dvt1, vt1 if n1 > 0 else None, True)):
+        if like is None and t is not None:
+            raise RuntimeError(f"magicdance_b200: {nm} given without the operand it is the gradient of")
+        dests.append(None if like is None else
+                     _dest(t, like.shape, torch.float16, q.device, nm, rows8=True, zero=zero))
+    dq, dk0, dvt0, dk1, dvt1 = dests
     lib = _lib.load()
     for t, nm in ((q, "q"), (dout, "dout")):
         _chk(t, torch.float16, nm)
@@ -587,22 +585,12 @@ def attention_backward(q, k0, vt0, n0, out, dout, lse, *, heads, d, batch, nq, k
     a.fwd = _attn_desc(q, k0, vt0, n0, heads=heads, d=d, batch=batch, nq=nq, out=out, kv0_batches=kv0_batches,
                        ldv0_batch=ldv0_batch, k1=k1, vt1=vt1, n1=n1, kv1_batches=kv1_batches, ldv1_batch=ldv1_batch,
                        bank_batches=bank_batches, scale=scale)
-    dev = q.device
-    for nm, (t, _) in given.items():
-        if t is not None:
-            _chk(t, torch.float16, nm)
-    dq = torch.empty(q.shape, dtype=torch.float16, device=dev) if out_dq is None else out_dq
-    dk0 = torch.empty(k0.shape, dtype=torch.float16, device=dev) if out_dk0 is None else out_dk0
-    dvt0 = torch.zeros(vt0.shape, dtype=torch.float16, device=dev) if out_dvt0 is None else out_dvt0
     a.dout, a.lddout, a.lse = dout.data_ptr(), dout.stride(0), lse.data_ptr()
     a.dq, a.lddq = dq.data_ptr(), dq.stride(0)
     a.dk0, a.lddk0, a.dvt0, a.lddvt0 = dk0.data_ptr(), dk0.stride(0), dvt0.data_ptr(), dvt0.stride(0)
-    dk1 = dvt1 = None
     if n1 > 0:
-        dk1 = torch.zeros(k1.shape, dtype=torch.float16, device=dev) if out_dk1 is None else out_dk1
-        dvt1 = torch.zeros(vt1.shape, dtype=torch.float16, device=dev) if out_dvt1 is None else out_dvt1
         a.dk1, a.lddk1, a.dvt1, a.lddvt1 = dk1.data_ptr(), dk1.stride(0), dvt1.data_ptr(), dvt1.stride(0)
-    ws = _workspace("attn_bwd", int(lib.mdb_attention_bwd_ws_floats(batch, heads, nq)), torch.float32, dev)
+    ws = _workspace("attn_bwd", int(lib.mdb_attention_bwd_ws_floats(batch, heads, nq)), torch.float32, q.device)
     a.ws = ws.data_ptr()
     _lib.check(lib.mdb_attention_bwd_f16(C.byref(a), _stream()), "attention_bwd_f16")
     return dq, dk0, dvt0, dk1, dvt1
@@ -673,22 +661,6 @@ def layernorm(x, gamma, beta, eps=1e-5, out=None):
     return out
 
 
-def _dx_out(t, shape, dtype, device, name):
-    """a dx destination of the norm backwards: `t` (contiguous fp16 / fp32) or a new tensor"""
-    t = _grad_out(t, shape, dtype, device, name)
-    assert t.is_contiguous(), name
-    return t
-
-
-def _param_grad(t, n, device, name):
-    """an fp32 [n] gradient destination of gamma / beta: `t` or a new tensor"""
-    if t is None:
-        t = torch.empty(n, dtype=torch.float32, device=device)
-    _chk(t, torch.float32, name)
-    assert t.is_contiguous() and t.numel() == n, (name, t.shape, n)
-    return t
-
-
 def groupnorm_backward(x1, gamma, beta, dy, *, batch, hw, eps, silu, x2=None, grads=("x", "gamma", "beta"),
                        dx_dtype=torch.float16, out_dx1=None, out_dx2=None, out_dgamma=None, out_dbeta=None,
                        accumulate=()):
@@ -718,22 +690,19 @@ def groupnorm_backward(x1, gamma, beta, dy, *, batch, hw, eps, silu, x2=None, gr
     acc = set(accumulate)
     dx1 = dx2 = dgamma = dbeta = None
     if "x" in grads:
-        dx1 = _dx_out(out_dx1, (batch * hw, c1), dx_dtype, dev, "out_dx1")
+        dx1 = _dest(out_dx1, (batch * hw, c1), dx_dtype, dev, "out_dx1", any_float=True, contiguous=True)
         d.dx1, d.dx1_dtype, d.dx1_accumulate = dx1.data_ptr(), _DTYPES[dx1.dtype], "x" in acc
         if x2 is not None:
-            dx2 = _dx_out(out_dx2, (batch * hw, c2), dx_dtype, dev, "out_dx2")
+            dx2 = _dest(out_dx2, (batch * hw, c2), dx_dtype, dev, "out_dx2", any_float=True, contiguous=True)
             d.dx2, d.dx2_dtype, d.dx2_accumulate = dx2.data_ptr(), _DTYPES[dx2.dtype], "x2" in acc
     if "gamma" in grads:
-        dgamma = _param_grad(out_dgamma, c1 + c2, dev, "out_dgamma")
+        dgamma = _dest(out_dgamma, (c1 + c2,), torch.float32, dev, "out_dgamma", contiguous=True, numel=True)
         d.dgamma, d.dgamma_accumulate = dgamma.data_ptr(), "gamma" in acc
     if "beta" in grads:
-        dbeta = _param_grad(out_dbeta, c1 + c2, dev, "out_dbeta")
+        dbeta = _dest(out_dbeta, (c1 + c2,), torch.float32, dev, "out_dbeta", contiguous=True, numel=True)
         d.dbeta, d.dbeta_accumulate = dbeta.data_ptr(), "beta" in acc
-    need = int(lib.mdb_groupnorm_bwd_ws_floats(C.byref(d)))
-    if need < 0:
-        _lib.check(need, "groupnorm_bwd_f16")
     # the statistics kernel's tickets must be zero at first use (_workspace(zero=True)); the kernels leave them so
-    d.ws = _workspace("gn_bwd", need, torch.float32, dev, zero=True).data_ptr()
+    d.ws = _bwd_ws(d, lib.mdb_groupnorm_bwd_ws_floats, "gn_bwd", dev, "groupnorm_bwd_f16", zero=True)
     _lib.check(lib.mdb_groupnorm_bwd_f16(C.byref(d), _stream()), "groupnorm_bwd_f16")
     return dx1, dx2, dgamma, dbeta
 
@@ -755,18 +724,15 @@ def layernorm_backward(x, gamma, dy, *, eps=1e-5, grads=("x", "gamma", "beta"), 
     acc = set(accumulate)
     dx = dgamma = dbeta = None
     if "x" in grads:
-        dx = _dx_out(out_dx, (rows, c), dx_dtype, dev, "out_dx")
+        dx = _dest(out_dx, (rows, c), dx_dtype, dev, "out_dx", any_float=True, contiguous=True)
         d.dx, d.dx_dtype, d.dx_accumulate = dx.data_ptr(), _DTYPES[dx.dtype], "x" in acc
     if "gamma" in grads:
-        dgamma = _param_grad(out_dgamma, c, dev, "out_dgamma")
+        dgamma = _dest(out_dgamma, (c,), torch.float32, dev, "out_dgamma", contiguous=True, numel=True)
         d.dgamma, d.dgamma_accumulate = dgamma.data_ptr(), "gamma" in acc
     if "beta" in grads:
-        dbeta = _param_grad(out_dbeta, c, dev, "out_dbeta")
+        dbeta = _dest(out_dbeta, (c,), torch.float32, dev, "out_dbeta", contiguous=True, numel=True)
         d.dbeta, d.dbeta_accumulate = dbeta.data_ptr(), "beta" in acc
-    need = int(lib.mdb_layernorm_bwd_ws_floats(C.byref(d)))
-    if need < 0:
-        _lib.check(need, "layernorm_bwd_f16")
-    d.ws = _workspace("ln_bwd", need, torch.float32, dev).data_ptr()
+    d.ws = _bwd_ws(d, lib.mdb_layernorm_bwd_ws_floats, "ln_bwd", dev, "layernorm_bwd_f16")
     _lib.check(lib.mdb_layernorm_bwd_f16(C.byref(d), _stream()), "layernorm_bwd_f16")
     return dx, dgamma, dbeta
 
@@ -809,8 +775,7 @@ class GroupNorm(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x1, gamma, beta, x2 = ctx.saved_tensors
-        need = ctx.needs_input_grad
-        grads = [nm for nm, want in (("x", need[0] or need[3]), ("gamma", need[1]), ("beta", need[2])) if want]
+        grads = _wanted(ctx, x=(0, 3), gamma=(1,), beta=(2,))
         dx1, dx2, dgamma, dbeta = groupnorm_backward(x1, gamma, beta, dy.contiguous(), x2=x2, grads=grads, **ctx.kw)
         return dx1, dgamma, dbeta, dx2, None, None, None, None
 
@@ -832,8 +797,7 @@ class LayerNorm(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x, gamma = ctx.saved_tensors
-        need = ctx.needs_input_grad
-        grads = [nm for nm, want in (("x", need[0]), ("gamma", need[1]), ("beta", need[2])) if want]
+        grads = _wanted(ctx, x=(0,), gamma=(1,), beta=(2,))
         dx, dgamma, dbeta = layernorm_backward(x, gamma, dy.contiguous(), eps=ctx.eps, grads=grads)
         return dx, dgamma, dbeta, None
 
@@ -1005,15 +969,6 @@ def flip_conv_weight(wt, *, cin, cout):
     return wt.reshape(cout, 3, 3, cin).flip(1, 2).permute(3, 1, 2, 0).contiguous().reshape(cin, 9 * cout)
 
 
-def _vec_out(t, n, dtype, device, name):
-    """a contiguous gradient destination of n elements: `t` or a new tensor"""
-    if t is None:
-        t = torch.empty(n, dtype=dtype, device=device)
-    _chk(t, dtype, name)
-    assert t.is_contiguous() and t.numel() == n, (name, t.shape, n)
-    return t
-
-
 def conv3x3_direct_backward(x, wt, dy, *, batch, h, w, cin, cout, stride=1, bias=None, silu=False, wt_t=None,
                             grads=("x", "w", "bias"), out_dx=None, out_dw=None, out_dbias=None, accumulate=()):
     """Gradients of y = conv3x3_direct(x, wt, bias, batch=, h=, w=, cin=, cout=, stride=, silu=[, residual=]) from
@@ -1044,21 +999,15 @@ def conv3x3_direct_backward(x, wt, dy, *, batch, h, w, cin, cout, stride=1, bias
             _chk(wt_t, torch.float16, "wt_t")
             assert wt_t.is_contiguous() and wt_t.numel() == wt.numel()
             d.wt_t = wt_t.data_ptr()
-        dx = torch.empty((batch * h * w, cin), dtype=torch.float16, device=dev) if out_dx is None else out_dx
-        _chk(dx, torch.float16, "out_dx")
-        assert dx.is_contiguous() and tuple(dx.shape) == (batch * h * w, cin), dx.shape
+        dx = _dest(out_dx, (batch * h * w, cin), torch.float16, dev, "out_dx", contiguous=True)
         d.dx = dx.data_ptr()
     if "w" in grads:
-        dw = out_dw if out_dw is not None else torch.empty((cout, cin, 3, 3), dtype=torch.float32, device=dev)
-        _vec_out(dw, cout * cin * 9, torch.float32, dev, "out_dw")
+        dw = _dest(out_dw, (cout, cin, 3, 3), torch.float32, dev, "out_dw", contiguous=True, numel=True)
         d.dw, d.dw_accumulate = dw.data_ptr(), "w" in acc
     if "bias" in grads:
-        dbias = _vec_out(out_dbias, cout, torch.float32, dev, "out_dbias")
+        dbias = _dest(out_dbias, (cout,), torch.float32, dev, "out_dbias", contiguous=True, numel=True)
         d.dbias, d.dbias_accumulate = dbias.data_ptr(), "bias" in acc
-    need = int(lib.mdb_conv3x3_direct_bwd_ws_floats(C.byref(d)))
-    if need < 0:
-        _lib.check(need, "conv3x3_direct_bwd_f16")
-    d.ws = _workspace("conv_bwd", need, torch.float32, dev).data_ptr()
+    d.ws = _bwd_ws(d, lib.mdb_conv3x3_direct_bwd_ws_floats, "conv_bwd", dev, "conv3x3_direct_bwd_f16")
     _lib.check(lib.mdb_conv3x3_direct_bwd_f16(C.byref(d), _stream()), "conv3x3_direct_bwd_f16")
     return dx, dw, dbias
 
@@ -1078,18 +1027,17 @@ class DirectConv3x3(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x, wt, w_param, bias = ctx.saved_tensors
-        need = ctx.needs_input_grad
-        grads = [nm for nm, want in (("x", need[0]), ("w", need[1] or need[2]), ("bias", need[3])) if want]
+        grads = _wanted(ctx, x=(0,), w=(1, 2), bias=(3,))
         dy = dy.contiguous()
         dx = dw = dbias = None
         if grads:
             dx, dw, dbias = conv3x3_direct_backward(x, wt, dy, bias=bias, grads=grads, **ctx.kw)
         g_wt = g_wp = None
-        if dw is not None:
+        if dw is not None:  # the kernel's dW is OIHW, the parameter's layout
             if w_param is not None:
                 g_wp = dw.view(w_param.shape)
             else:
-                g_wt = dw.permute(0, 2, 3, 1).reshape(wt.shape).to(wt.dtype)
+                g_wt = pack_conv_weight(dw).view(wt.shape)
         return dx, g_wt, g_wp, dbias, dy if ctx.has_residual else None, *(None,) * 7
 
 
@@ -1118,15 +1066,11 @@ def skinny_linear_backward(x, w, dy, *, silu_in=False, grads=("x", "w", "bias"),
     acc = set(accumulate)
     dx = dw = dbias = None
     if "x" in grads:
-        dx = _grad_out(out_dx, (rows, k), torch.float32, dev, "out_dx")
-        _chk(dx, torch.float32, "out_dx")
-        assert dx.is_contiguous()
+        dx = _dest(out_dx, (rows, k), torch.float32, dev, "out_dx", contiguous=True)
     if "w" in grads:
-        dw = _grad_out(out_dw, (n, k), torch.float32, dev, "out_dw")
-        _chk(dw, torch.float32, "out_dw")
-        assert dw.is_contiguous()
+        dw = _dest(out_dw, (n, k), torch.float32, dev, "out_dw", contiguous=True)
     if "bias" in grads:
-        dbias = _vec_out(out_dbias, n, torch.float32, dev, "out_dbias")
+        dbias = _dest(out_dbias, (n,), torch.float32, dev, "out_dbias", contiguous=True, numel=True)
     for r0 in range(0, rows, SKINNY_MAX_ROWS):
         d = _lib.SkinnyBwdDesc()
         d.x, d.w, d.dy = x[r0:].data_ptr(), w.data_ptr(), dy[r0:].data_ptr()
@@ -1137,10 +1081,7 @@ def skinny_linear_backward(x, w, dy, *, silu_in=False, grads=("x", "w", "bias"),
             d.dw, d.dw_accumulate = dw.data_ptr(), r0 > 0 or "w" in acc
         if dbias is not None:
             d.dbias, d.dbias_accumulate = dbias.data_ptr(), r0 > 0 or "bias" in acc
-        need = int(lib.mdb_skinny_linear_bwd_ws_floats(C.byref(d)))
-        if need < 0:
-            _lib.check(need, "skinny_linear_bwd_f32")
-        d.ws = _workspace("skinny_bwd", need, torch.float32, dev).data_ptr()
+        d.ws = _bwd_ws(d, lib.mdb_skinny_linear_bwd_ws_floats, "skinny_bwd", dev, "skinny_linear_bwd_f32")
         _lib.check(lib.mdb_skinny_linear_bwd_f32(C.byref(d), _stream()), "skinny_linear_bwd_f32")
     return dx, dw, dbias
 
@@ -1158,17 +1099,11 @@ class SkinnyLinear(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         x, w, w_param = ctx.saved_tensors
-        need = ctx.needs_input_grad
-        grads = [nm for nm, want in (("x", need[0]), ("w", need[1] or need[2]), ("bias", need[3])) if want]
+        grads = _wanted(ctx, x=(0,), w=(1, 2), bias=(3,))
         dx = dw = dbias = None
         if grads:
             dx, dw, dbias = skinny_linear_backward(x, w, dout.contiguous(), silu_in=ctx.silu_in, grads=grads)
-        g_w = g_wp = None
-        if dw is not None:
-            if w_param is not None:
-                g_wp = dw.view(w_param.shape)
-            else:
-                g_w = dw.to(w.dtype)
+        g_w, g_wp = _route_grad(dw, w, w_param)
         return dx, g_w, g_wp, dbias, None
 
 
@@ -1185,8 +1120,7 @@ def upsample2x_backward(dy, *, batch, h, w, c, dx_dtype=torch.float16, out_dx=No
     lib = _lib.load()
     _chk(dy, torch.float16, "dy")
     assert dy.is_contiguous() and tuple(dy.shape) == (batch * 4 * h * w, c), dy.shape
-    dx = _grad_out(out_dx, (batch * h * w, c), dx_dtype, dy.device, "out_dx")
-    assert dx.is_contiguous()
+    dx = _dest(out_dx, (batch * h * w, c), dx_dtype, dy.device, "out_dx", any_float=True, contiguous=True)
     _lib.check(lib.mdb_upsample2x_bwd_f16(dy.data_ptr(), dx.data_ptr(), _DTYPES[dx.dtype], int(accumulate), batch, h,
                                           w, c, _stream()), "upsample2x_bwd_f16")
     return dx

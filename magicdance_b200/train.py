@@ -82,11 +82,6 @@ def _input(t, gs):
 # ------------------------------------------------------------------------------------------------
 # weights
 # ------------------------------------------------------------------------------------------------
-def _conv_pack(w):
-    """Conv2d OIHW -> [O][kh][kw][I] viewed as [O, 9*I] (engine.pack_conv3x3's layout)"""
-    return w.permute(0, 2, 3, 1).reshape(w.shape[0], -1)
-
-
 def _mat(w):
     """Linear (out, in) as it is; a 1x1 Conv2d (O, I, 1, 1) viewed as (O, I)"""
     return w.reshape(w.shape[0], -1)
@@ -126,7 +121,7 @@ class _Weights:
         return hit[1], hit[2]
 
     def conv(self, name):
-        return self.packed((name, "conv"), [name], lambda w: w, _conv_pack)
+        return self.packed((name, "conv"), [name], lambda w: w, ops.pack_conv_weight)
 
     def mat(self, name):
         return self.packed((name, "mat"), [name], _mat)

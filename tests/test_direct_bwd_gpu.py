@@ -62,11 +62,6 @@ def _nhwc(t):
     return t.permute(0, 2, 3, 1).reshape(-1, t.shape[1])
 
 
-def _conv_pack(w):
-    """Conv2d OIHW -> fp16 [O][kh][kw][I], detached (the kernels' layout)"""
-    return w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1).half().contiguous()
-
-
 def _check(errs, sd, p, r):
     for k in sd:
         assert p[k].grad.shape == r[k].grad.shape and p[k].grad.dtype == torch.float32, k
@@ -106,13 +101,13 @@ def _pose_hint_path():
     for i in range(7):
         cin, cout, st = chans[i], chans[i + 1], strides[i]
         wp = p[f"input_hint_block.{2 * i}.weight"]
-        h = ops.direct_conv3x3(h, _conv_pack(wp), w_param=wp, bias=p[f"input_hint_block.{2 * i}.bias"], batch=b,
+        h = ops.direct_conv3x3(h, ops.pack_conv_weight(wp), w_param=wp, bias=p[f"input_hint_block.{2 * i}.bias"], batch=b,
                                h=hh, w=hh, cin=cin, cout=cout, stride=st, silu=True)
         hh = (hh - 1) // st + 1
     wl = p["input_hint_block.14.weight"]
-    hint = ops.tc_gemm(h, _conv_pack(wl), w_param=wl, bias=p["input_hint_block.14.bias"], conv=(b, hh, hh, 256))
+    hint = ops.tc_gemm(h, ops.pack_conv_weight(wl), w_param=wl, bias=p["input_hint_block.14.bias"], conv=(b, hh, hh, 256))
     wc = p["input_blocks.0.0.weight"]
-    out = ops.direct_conv3x3(ops.nchw_to_nhwc(xn), _conv_pack(wc), w_param=wc, bias=p["input_blocks.0.0.bias"],
+    out = ops.direct_conv3x3(ops.nchw_to_nhwc(xn), ops.pack_conv_weight(wc), w_param=wc, bias=p["input_blocks.0.0.bias"],
                              residual=hint, batch=b, h=lat, w=lat, cin=4, cout=320)
     (out.float() * g).sum().backward()
 
@@ -162,11 +157,11 @@ def _time_path(t):
     bias = (emb_all[:, :c] + p[pre + "in_layers.2.bias"]).contiguous()
     a = ops.group_norm(xs, p[pre + "in_layers.0.weight"], p[pre + "in_layers.0.bias"], batch=b, hw=hw, eps=1e-5,
                        silu=True)
-    a = ops.tc_gemm(a, _conv_pack(p[pre + "in_layers.2.weight"]), w_param=p[pre + "in_layers.2.weight"], bias=bias,
+    a = ops.tc_gemm(a, ops.pack_conv_weight(p[pre + "in_layers.2.weight"]), w_param=p[pre + "in_layers.2.weight"], bias=bias,
                     bias_batch_stride=c, rows_per_batch=hw, conv=(b, hh, ww, c))
     a = ops.group_norm(a, p[pre + "out_layers.0.weight"], p[pre + "out_layers.0.bias"], batch=b, hw=hw, eps=1e-5,
                        silu=True)
-    out = ops.tc_gemm(a, _conv_pack(p[pre + "out_layers.3.weight"]), w_param=p[pre + "out_layers.3.weight"],
+    out = ops.tc_gemm(a, ops.pack_conv_weight(p[pre + "out_layers.3.weight"]), w_param=p[pre + "out_layers.3.weight"],
                       bias=p[pre + "out_layers.3.bias"], residual=xs, conv=(b, hh, ww, c))
     (out.float() * g).sum().backward()
     assert not other["w"].grad.any() and not other["b"].grad.any()  # the other block's slice gets exactly zero
@@ -199,9 +194,9 @@ def _head_and_upsample():
     p = _leaves(sd)
     hs, us = h.clone().requires_grad_(), u.clone().requires_grad_()
     a = ops.group_norm(hs, p["out.0.weight"], p["out.0.bias"], batch=b, hw=hh * hh, eps=1e-5, silu=True)
-    eps_out = ops.direct_conv3x3(a, _conv_pack(w_out), batch=b, h=hh, w=hh, cin=c, cout=4)
+    eps_out = ops.direct_conv3x3(a, ops.pack_conv_weight(w_out), batch=b, h=hh, w=hh, cin=c, cout=4)
     up = ops.upsample_2x(us, batch=b, h=lo, w=lo, c=cu)
-    y = ops.tc_gemm(up, _conv_pack(p["up.conv.weight"]), w_param=p["up.conv.weight"], bias=p["up.conv.bias"],
+    y = ops.tc_gemm(up, ops.pack_conv_weight(p["up.conv.weight"]), w_param=p["up.conv.weight"], bias=p["up.conv.bias"],
                     conv=(b, hh, hh, cu))
     ((eps_out.float() * g1).sum() + (y.float() * g2).sum()).backward()
 

@@ -57,11 +57,6 @@ def _nhwc(t):
     return t.permute(0, 2, 3, 1).reshape(-1, t.shape[1])
 
 
-def _conv_pack(w):
-    """Conv2d OIHW -> fp16 [O][kh][kw][I], detached (the kernels' layout)"""
-    return w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1).half().contiguous()
-
-
 def _check(errs):
     print({k: f"{v:.2e}" for k, v in errs.items()})
     assert max(errs.values()) <= 1e-2, errs
@@ -95,13 +90,13 @@ def _resblock():
     a = ops.group_norm(xs[0], p["in_layers.0.weight"], p["in_layers.0.bias"], batch=b, hw=hw, eps=1e-5, silu=True,
                        x2=xs[1])
     e = F.linear(F.silu(emb), p["emb_layers.1.weight"], p["emb_layers.1.bias"]) + p["in_layers.2.bias"]
-    a = ops.tc_gemm(a, _conv_pack(p["in_layers.2.weight"]), w_param=p["in_layers.2.weight"], bias=e.contiguous(),
+    a = ops.tc_gemm(a, ops.pack_conv_weight(p["in_layers.2.weight"]), w_param=p["in_layers.2.weight"], bias=e.contiguous(),
                     bias_batch_stride=co, rows_per_batch=hw, conv=(b, hh, ww, ci))
     a = ops.group_norm(a, p["out_layers.0.weight"], p["out_layers.0.bias"], batch=b, hw=hw, eps=1e-5, silu=True)
     wsk = p["skip_connection.weight"]
     res = ops.tc_gemm(xs[0], wsk.detach().view(co, ci).half(), w_param=wsk.view(co, ci), a2=xs[1],
                       bias=p["skip_connection.bias"])
-    out = ops.tc_gemm(a, _conv_pack(p["out_layers.3.weight"]), w_param=p["out_layers.3.weight"],
+    out = ops.tc_gemm(a, ops.pack_conv_weight(p["out_layers.3.weight"]), w_param=p["out_layers.3.weight"],
                       bias=p["out_layers.3.bias"], residual=res, conv=(b, hh, ww, co))
     (out.float() * g).sum().backward()
 
